@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- the headline measurement for the Snappy raw-block hot path.
 
-Workload (BASELINE.json configs[1]): `--blocks` (default 1,048,576) independent
+Workload (BASELINE.json configs[1]): `--blocks` (default 524,288 = 32 GiB) independent
 64KB synthetic text blocks per GPU, block i = T[off_i : off_i+65536] with
 T = alice29 || asyoulik || lcet10 || plrabn12 and off_i = (i*65521) mod (|T|-65536)
 (SURVEY.md 8d). One step = compress every block (K1) then decompress every
@@ -102,7 +102,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler(threading.Thread):
@@ -368,6 +368,10 @@ def run_ours(args, rank, local_rank, world):
     u_rank = blocks * BLOCK
     u_all = u_rank * world
 
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, "rank%d" % rank),
+                     t_c, t_clen, t_out, t_dlen, t_st, blocks, wave, nwaves, first_block)
+
     # ---------------- e2e: host buffers through the C ABI (H2D/D2H inside the timed region)
     e2e = None
     if not args.no_e2e:
@@ -394,13 +398,6 @@ def run_ours(args, rank, local_rank, world):
     k1_bytes = (u_rank + comp_bytes) * args.steps          # algorithmic bytes moved by K1 launches
     k1_achieved = k1_bytes / (ms_c / 1e3) / 1e9
     k2_achieved = k1_bytes / (ms_d / 1e3) / 1e9
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "k1_traffic.json")
-    if os.path.exists(tp):
-        try:
-            traffic = json.load(open(tp)).get("dram_bytes_per_block") * min(wave, blocks)   # per launch
-        except Exception:  # noqa: BLE001
-            traffic = None
     line = {
         "metric": METRIC, "value": value, "unit": "GB/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_tot / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -414,7 +411,7 @@ def run_ours(args, rank, local_rank, world):
         "compress_gbs": u_all * args.steps / (ms_cmax / 1e3) / 1e9,
         "decompress_gbs": u_all * args.steps / (ms_dmax / 1e3) / 1e9,
         "roofline": {"bound": "hbm", "kernel": "k1_m7_kernel (K1 compress)", "achieved": k1_achieved, "peak": peak, "unit": "GB/s",
-                     "frac": k1_achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                     "frac": k1_achieved / peak, "traffic": None, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": (u_rank + comp_bytes) / nwaves,
                      "k2_decompress_kernel": {"achieved": k2_achieved, "frac": k2_achieved / peak}},
         "clocks": clocks, "gpu_launches": int(launches), "compressed_bytes_all_ranks": comp_all,
@@ -427,6 +424,32 @@ def run_ours(args, rank, local_rank, world):
         from oracle import oracle as orc
         line["cpu_baseline"], _ = cpu_baseline_report(orc, text, 12.0)
     print(json.dumps(line), flush=True)
+
+
+def dump_outputs(out_dir, t_c, t_clen, t_out, t_dlen, t_st, blocks, wave, nwaves, first_block, samples=48, seed=0):
+    """Write what the last timed step returned to its caller as .npy files (~30 MB at most): the compressed
+    length of every block, and for a fixed, seeded sample of the last wave's blocks their compressed streams (zero
+    padded to the slot stride), their decompressed bytes, lengths and decode statuses."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    lo = (nwaves - 1) * wave
+    cnt = blocks - lo
+    idx = np.sort(np.random.default_rng(seed).choice(cnt, size=min(samples, cnt), replace=False))
+    t_idx = torch.from_numpy(idx).to(t_c.device)
+    clen = t_clen[lo:lo + cnt].cpu().numpy()
+    comp = t_c[:cnt * STRIDE].view(cnt, STRIDE)[t_idx].cpu().numpy()
+    comp[np.arange(STRIDE)[None, :] >= clen[idx][:, None]] = 0            # slot bytes past the stream are not output
+    out = {
+        "compressed_lengths": t_clen.cpu().numpy(),
+        "sample_block_index": first_block + lo + idx,
+        "compressed_sample": comp,
+        "decompressed_sample": t_out[:cnt * BLOCK].view(cnt, BLOCK)[t_idx].cpu().numpy(),
+        "decompressed_lengths": t_dlen[:cnt].cpu().numpy(),
+        "decode_status": t_st.view(wave, 4)[:cnt, 0].cpu().numpy(),
+    }
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64 if name == "sample_block_index" else np.float32))
 
 
 def run_e2e(args, snap, L, torch, dev, t_in, t_clen, rank, world):
@@ -685,7 +708,7 @@ def run_frame_shard(args, rank, local_rank, world):
 
 def run_frame(args, local_rank):
     """--workload frame: BASELINE configs[3], FrameEncoder/FrameDecoder over a long synthetic stream on one GPU,
-    device resident, in waves (the 256 GiB stream and its ~155 GiB of frames do not fit 180 GB at once): every wave
+    device resident, in waves (the 256 GiB stream and its ~155 GiB of frames do not fit 80 GB at once): every wave
     is frame-encoded (K1 with the chunk CRC in the emitter, scan, gather) and decoded again (header parse from the
     encoder's chunk index, K2, CRC verify). The first pass checks decode(encode(x)) == x for every wave."""
     import torch
@@ -781,7 +804,7 @@ def run_frame(args, local_rank):
         "value": 2 * u * args.steps / ((ms_e + ms_d) / 1e3) / 1e9, "unit": "GB/s", "n_gpus": 1, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": (ms_e + ms_d) / args.steps, "higher_is_better": True, "dtype": "u8",
         "data": "synthetic", "side_measurement": True,
-        "config": {"workload": "FrameEncoder/FrameDecoder over a %.0f GiB synthetic text stream in %d waves of %.1f GiB on 1 B200 (BASELINE configs[3])"
+        "config": {"workload": "FrameEncoder/FrameDecoder over a %.0f GiB synthetic text stream in %d waves of %.1f GiB on 1 GPU (BASELINE configs[3])"
                                % (u / 2**30, nwaves, wave_bytes / 2**30), "stream_bytes": stream_bytes, "ratio": stream_bytes / u,
                    "input_pool_waves": pool_waves,
                    "parity": "every wave: decode(encode(x)) == x on device, statuses Ok; first 4 chunks == oracle FrameEncoder bytes"},
@@ -864,10 +887,11 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--blocks", type=int, default=1 << 20, help="64KB blocks per GPU (BASELINE configs[1]: 1M)")
+    ap.add_argument("--blocks", type=int, default=1 << 19,
+                    help="64KB blocks per GPU (512K = 32 GiB: inputs plus wave buffers fit an 80 GB H100)")
     ap.add_argument("--wave", type=int, default=1 << 17, help="blocks per kernel launch")
     ap.add_argument("--e2e-blocks", type=int, default=1 << 18)
-    ap.add_argument("--e2e-batches", type=int, default=1, help="e2e: batches pipelined through compress and decompress from two host threads (1 = sequential phases; measured: 8 batches 33.3, 16 batches 35.9, sequential 37.9 GB/s -- K1 owns every SM, so the overlap buys nothing)")
+    ap.add_argument("--e2e-batches", type=int, default=1, help="e2e: batches pipelined through compress and decompress from two host threads (1 = sequential phases)")
     ap.add_argument("--parity-samples", type=int, default=48)
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
@@ -879,10 +903,16 @@ def main():
     ap.add_argument("--workload", default="text-roundtrip", choices=["text-roundtrip", "urls-decompress", "frame", "frame-shard"],
                     help="side measurements: urls-decompress = BASELINE configs[2]; frame = configs[3] (--gib, default 256); "
                          "frame-shard = configs[4] (--gib total over all ranks, default 1024)")
-    ap.add_argument("--urls-gib", type=float, default=64.0)
+    ap.add_argument("--urls-gib", type=float, default=32.0, help="uncompressed GiB of tiled urls.10K (output + input fit 80 GB)")
     ap.add_argument("--gib", type=float, default=None)
     ap.add_argument("--wave-gib", type=float, default=None)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="text-roundtrip: after the timed steps, write the last step's outputs to DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.workload != "text-roundtrip" or args.impl != "ours"):
+        ap.error("--dump-outputs applies to the default text-roundtrip workload of --impl ours")
     if args.warmup < 3 and args.workload != "frame-shard":
         args.warmup = 3          # frame-shard steps are whole-stream passes (hundreds of waves each): --warmup 1 is accepted there
     rank = int(os.environ.get("RANK", "0"))

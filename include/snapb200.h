@@ -1,12 +1,12 @@
 /*
- * snapb200.h -- C ABI of the B200-native Snappy codec (libsnapb200.so).
+ * snapb200.h -- C ABI of the GPU-native (H100, sm_90a) Snappy codec (libsnapb200.so).
  *
  * This is the drop-in boundary for rust-snappy's raw/frame hot path: a Rust
  * `snap` shim (see INTEGRATION.md, rust/) binds exactly these symbols. Each
  * entry point cites the reference interface it replaces (paths relative to the
  * rust-snappy checkout). Plain pointers and sizes only -- no torch/CUDA types.
  *
- * All work is done by sm_100a CUDA kernels; there is NO CPU fallback. When no
+ * All work is done by sm_90a CUDA kernels; there is NO CPU fallback. When no
  * CUDA device is usable every compute call returns SB_E_NO_DEVICE.
  */
 #ifndef SNAPB200_H

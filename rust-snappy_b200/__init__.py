@@ -1,5 +1,5 @@
 """rust-snappy_b200 -- host-side mirror of the `snap` crate's public API over
-the C ABI of libsnapb200.so (hand-written sm_100a kernels; no CPU fallback).
+the C ABI of libsnapb200.so (hand-written sm_90a kernels; no CPU fallback).
 
     snap::raw::{Encoder, Decoder, max_compress_len, decompress_len} -> .raw
     snap::write::FrameEncoder                                      -> .write

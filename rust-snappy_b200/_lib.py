@@ -1,7 +1,7 @@
 """ctypes binding of libsnapb200.so (the C ABI in include/snapb200.h).
 
 There is no fallback: if the shared library is missing this module raises, and
-if no B200 is visible every compute call returns SB_E_NO_DEVICE which surfaces as
+if no H100 (sm_90a) is visible every compute call returns SB_E_NO_DEVICE which surfaces as
 `NoDevice`.
 """
 import ctypes as C

@@ -1,4 +1,4 @@
-// common.cuh -- shared definitions for the sm_100a Snappy kernels.
+// common.cuh -- shared definitions for the sm_90a Snappy kernels.
 #pragma once
 #include "simt.h"
 #include "../../include/snapb200.h"

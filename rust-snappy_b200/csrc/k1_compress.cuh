@@ -29,10 +29,10 @@
 //    from a ring, 32 at a time: literal/copy tag sizes, a warp scan for output
 //    offsets, tags and literal bytes written straight to HBM (evict-first).
 //
-// Measured and rejected in round 2 (profiles/r2_k1_variants_ab.txt): 64-position steps, unaligned windows,
-// speculative slot reads for the L2-table chains, an mbarrier wake-up for the emitter, and a second-generation
-// parser with exact windows and pipelined candidate evaluation. The one-pair-per-CTA layouts of round 1
-// (shared-memory window, pipelined parser warps) are gone as well; their numbers are in DESIGN.md.
+// Tried and rejected (slower on hardware): 64-position steps, unaligned windows, speculative slot reads for the
+// L2-table chains, an mbarrier wake-up for the emitter, and a second-generation parser with exact windows and
+// pipelined candidate evaluation. The one-pair-per-CTA layouts of round 1 (shared-memory window, pipelined parser
+// warps) are gone as well (DESIGN.md section 4).
 #pragma once
 #include "common.cuh"
 #include "k3_crc32c.cuh"

@@ -1,6 +1,6 @@
 // simt.h -- thin portability layer for the kernel bodies.
 //
-// Under nvcc the wrappers are the sm_100a intrinsics, nothing more. Under
+// Under nvcc the wrappers are the sm_90a intrinsics, nothing more. Under
 // -DSB_EMU (tests/emu only) the same kernel bodies are compiled by g++ against a
 // fiber-based warp emulator so their LOGIC can be checked on a machine without a
 // GPU. The emulator is test tooling: the product library is only ever built

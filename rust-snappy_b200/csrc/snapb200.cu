@@ -1,6 +1,6 @@
-// snapb200.cu -- libsnapb200.so: sm_100a kernels + the C ABI of include/snapb200.h.
+// snapb200.cu -- libsnapb200.so: sm_90a (H100) kernels + the C ABI of include/snapb200.h.
 // Built by __graft_entry__.build() with
-//   nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared -Xcompiler -fPIC
+//   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC
 // There is no CPU execution path in this library: every compute entry point
 // launches the kernels below and fails with SB_E_NO_DEVICE when it cannot.
 #include <cuda_runtime.h>
@@ -50,7 +50,9 @@ __global__ void __launch_bounds__(256) k6_generate_kernel(sbk::GenPlan g) { sbk:
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
 const int K2_DEFAULT_CTAS_PER_SM = 16;
-const int K1_DEFAULT_NG = 5;
+// H100 (50 MB L2): the 7 shared-memory chains per SM already keep more input windows hot than L2 holds, and every
+// L2-table chain adds its table and window on top; 7 + 0 chains measured fastest (DESIGN.md section 5)
+const int K1_DEFAULT_NG = 0;
 
 int fail(sb_error* e, uint32_t code, uint64_t a = 0, uint64_t b = 0, uint64_t c = 0) {
     if (e) { e->code = code; e->_pad = 0; e->a = a; e->b = b; e->c = c; }
@@ -210,7 +212,7 @@ int launch_k2(Ctx& c, const sb_batch& b, cudaStream_t st, sb_error* err) {
     const unsigned wpb = 4;
     uint64_t blocks = ((uint64_t)b.count + wpb - 1) / wpb;
     // resident CTAs per SM: each warp keeps a 64KB output history alive, and copy sources are
-    // re-read from it -- too many streams in flight and the history falls out of the 126MB L2
+    // re-read from it -- too many streams in flight and the history falls out of the 50MB L2
     static const int per_sm = getenv("SNAPB200_K2_CTAS") ? atoi(getenv("SNAPB200_K2_CTAS")) : K2_DEFAULT_CTAS_PER_SM;
     unsigned grid = (unsigned)(per_sm * c.sms);
     if (grid > blocks) grid = (unsigned)blocks;
@@ -382,7 +384,7 @@ int decode_payload_phase(Ctx& c, const sbk::DecodePlan& p, cudaStream_t st, sb_e
 // =========================================================================
 extern "C" {
 
-const char* sb_version(void) { return "snapb200 0.2 (sm_100a)"; }
+const char* sb_version(void) { return "snapb200 0.2 (sm_90a)"; }
 uint64_t sb_launch_count(void) { return g_launches.load(); }
 uint64_t sb_alloc_count(void) { return g_allocs.load(); }
 

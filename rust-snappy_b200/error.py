@@ -65,5 +65,5 @@ def from_c(e):
     if code == 100:
         return UnexpectedEof("failed to fill whole buffer")
     if code == 200:
-        return NoDevice("no usable CUDA device (sm_100a) for libsnapb200 -- there is no CPU fallback")
+        return NoDevice("no usable CUDA device (sm_90a) for libsnapb200 -- there is no CPU fallback")
     return RuntimeError("libsnapb200 failure code=%d a=%d b=%d c=%d" % (code, e.a, e.b, e.c))

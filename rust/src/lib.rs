@@ -1,6 +1,6 @@
 //! `snap` API surface (raw::{Encoder, Decoder, max_compress_len, decompress_len},
 //! write::FrameEncoder, read::{FrameDecoder, FrameEncoder}, Error) forwarding the
-//! hot path to the B200 kernels through the C ABI of include/snapb200.h.
+//! hot path to the H100 kernels through the C ABI of include/snapb200.h.
 //! Host code stays in Rust; nothing here compresses on the CPU.
 use std::io;
 

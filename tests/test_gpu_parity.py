@@ -454,7 +454,7 @@ units = adversarial_blocks()
 for name in ("alice29.txt", "html", "urls.10K", "kppkn.gtb", "fireworks.jpeg", "geo.protodata"):
     d = corpus(name)
     units += [d[i:i + 65536] for i in range(0, len(d), 65536)]
-units = units * 30                     # > 148 x 14 units so every chain of every SM takes one or more
+units = units * 30                     # > 132 x 14 units so every chain of every SM takes one or more
 got = gpu_helpers.compress_batch_host(units)
 print("DIGEST", len(units), hashlib.sha256(b"".join(len(g).to_bytes(4, "little") + g for g in got)).hexdigest())
 """

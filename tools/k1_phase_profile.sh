@@ -4,7 +4,7 @@
 set -e
 cd "$(dirname "$0")/.."
 mkdir -p gpurun_out
-nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -shared -Xcompiler -fPIC -DK1_PROFILE \
+nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -shared -Xcompiler -fPIC -DK1_PROFILE \
      -o gpurun_out/libsnapb200_prof.so rust-snappy_b200/csrc/snapb200.cu
 SNAPB200_LIB=$PWD/gpurun_out/libsnapb200_prof.so python - <<'PY'
 import ctypes as C, json, os, sys
