@@ -46,7 +46,11 @@ __device__ unsigned long long g_k1_prof[16];
 #define K1_PROF_ARGS , unsigned long long* k1_acc, long long& k1_t0
 #define K1_PROF_PASS , k1_acc, k1_t0
 #define K1_PROF_FLUSH do { if (sbk::lane_id() == 0) for (int _i = 0; _i < 12; _i++) atomicAdd(&g_k1_prof[_i], k1_acc[_i]); } while (0)
+// [12 + s]: parser warps the hardware placed on scheduler s (%warpid & 3), one count per warp and launch
+#define K1_PROF_CENSUS(is_parser) do { unsigned _hw; asm volatile("mov.u32 %0, %%warpid;" : "=r"(_hw)); \
+    if ((is_parser) && sbk::lane_id() == 0) atomicAdd(&g_k1_prof[12 + (_hw & 3u)], 1ull); } while (0)
 #else
+#define K1_PROF_CENSUS(is_parser) do { } while (0)
 #define K1_TICK(slot) do { } while (0)
 #define K1_PROF_DECL
 #define K1_PROF_ARGS
@@ -577,12 +581,13 @@ SB_DEVICE uint32_t k1_emit_block(const uint8_t* win, uint8_t* out, uint32_t d, c
 // Unit limits (include/snapb200.h): a unit is one block, n <= 65536, and its output slot must hold
 // max_compress_len(n) bytes; a unit that violates either is skipped with out_lens = 0 and, when the batch has a
 // status array, TooBig / BufferTooSmall with the reference's payloads (src/compress.rs:104-117).
-template <bool GT>
+// The role is a template argument so that the parser's code does not keep the emitter's state (ring tail, output
+// pointer) live across the parse: with one shared body the 7 + 5 and 7 + 7 kernels spill under their register caps.
+template <bool GT, bool parser>
 SB_DEVICE void k1_chain(const BatchDesc& b, uint32_t flags, uint16_t* table, const K1Ring& ring, uint32_t* ctrl,
                         uint32_t* work, unsigned bar, uint32_t* crcs, const uint32_t* crc_tab) {
-    const unsigned lane = lane_id(), wid = warp_id();
-    const bool parser = (wid & 1u) == 0;
-    const unsigned pt = (wid & 1u) * 32 + lane;                        // thread index within the pair
+    const unsigned lane = lane_id();
+    const unsigned pt = (parser ? 0u : 32u) + lane;                    // thread index within the pair
     uint32_t tail = 0;                // emitter's private ring counter (never reset)
     if (pt == 0) { ctrl[0] = 0; ctrl[1] = 0; ctrl[6] = 0; ctrl[7] = 0; }
     for (;;) {
@@ -649,7 +654,15 @@ template <int NC, int NG>
 SB_DEVICE void k1_compress_body_multi(const BatchDesc& b, uint32_t flags, uint64_t* ring_scratch, uint16_t* gtables,
                                       uint32_t* work, uint32_t* crcs) {
     uint8_t* sm = smem();
-    const unsigned c = warp_id() >> 1;                                 // chain within the CTA
+    // Roles: with P chains in the CTA, warp c < P parses chain c and warp P + c emits for it. A warp is issued by the
+    // scheduler (sub-partition) of its warp slot mod 4 and a CTA's warps take consecutive slots, so the parsers, which
+    // bound the kernel, spread over all four schedulers (2/2/2/1 for P = 7). Pairing warps 2c / 2c + 1 would put every
+    // parser on two schedulers and leave the other two to emitters that mostly sleep. A pair's named barrier does not
+    // need its two warps to be adjacent.
+    const unsigned P = block_dim() / 64, w = warp_id();
+    const bool parser = w < P;
+    const unsigned c = parser ? w : w - P;                             // chain within the CTA
+    K1_PROF_CENSUS(parser);
     uint32_t* ctrl = (uint32_t*)(sm + (size_t)NC * K1_TABLE_BYTES + c * 64);
     uint32_t* crc_tab = (uint32_t*)(sm + (size_t)NC * K1_TABLE_BYTES + (size_t)(NC + NG) * 64);
     if (crcs) { k3_build_table1(crc_tab, thread_idx(), block_dim()); syncthreads(); }
@@ -657,8 +670,15 @@ SB_DEVICE void k1_compress_body_multi(const BatchDesc& b, uint32_t flags, uint64
     ring.size = K1_RING_GW;
     ring.ev = ring_scratch + ((size_t)block_idx() * (NC + NG) + c) * K1_RING_GW;
     ring.ctrl = ctrl;
-    if (NG == 0 || c < NC) k1_chain<false>(b, flags, (uint16_t*)(sm + (size_t)c * K1_TABLE_BYTES), ring, ctrl, work, 1 + c, crcs, crc_tab);
-    else k1_chain<true>(b, flags, gtables + ((size_t)block_idx() * NG + (c - NC)) * (K1_TABLE_BYTES / 2), ring, ctrl, work, 1 + c, crcs, crc_tab);
+    if (NG == 0 || c < NC) {
+        uint16_t* table = (uint16_t*)(sm + (size_t)c * K1_TABLE_BYTES);
+        if (parser) k1_chain<false, true>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
+        else k1_chain<false, false>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
+    } else {
+        uint16_t* table = gtables + ((size_t)block_idx() * NG + (c - NC)) * (K1_TABLE_BYTES / 2);
+        if (parser) k1_chain<true, true>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
+        else k1_chain<true, false>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
+    }
 }
 
 }  // namespace sbk

@@ -188,10 +188,14 @@ int launch_k1(Ctx& c, const sb_batch& b, uint32_t flags, uint32_t* crcs, cudaStr
     // SNAPB200_K1_NG = chains per SM with L2-resident tables next to the 7 shared-memory ones (0..7)
     static const int ng_env = getenv("SNAPB200_K1_NG") ? atoi(getenv("SNAPB200_K1_NG")) : K1_DEFAULT_NG;
     const unsigned ng = ng_env < 0 ? 0 : ng_env > K1_MAX_NG ? K1_MAX_NG : (unsigned)ng_env;
+    // SNAPB200_K1_CHAINS = cap on chains per SM (1..7 + NG; unset = no cap). Chains fill the shared-memory tables
+    // first, so a cap of 7 or less runs that many shared-memory chains alone (each one fewer measured slower on H100)
+    static const int cap_env = getenv("SNAPB200_K1_CHAINS") ? atoi(getenv("SNAPB200_K1_CHAINS")) : 0;
+    const unsigned cap = cap_env > 0 && (unsigned)cap_env < 7 + ng ? (unsigned)cap_env : 7 + ng;
     // small batches spread over the SMs first (one shared-memory-table chain per SM is the fastest a block can
     // run); only batches with more units than that stack chains on an SM, L2-table chains last
     unsigned chains = (unsigned)(((uint64_t)b.count + c.sms - 1) / c.sms);
-    if (chains > 7 + ng) chains = 7 + ng;
+    if (chains > cap) chains = cap;
     unsigned mg = (unsigned)c.sms;
     if (mg > b.count) mg = b.count;
     std::lock_guard<std::mutex> k1lk(c.k1_mu);
