@@ -165,10 +165,13 @@ int sb_frame_encode_device_ws(const uint8_t* d_in, uint64_t n, uint8_t* d_out, u
                               uint64_t* d_chunk_offs, sb_frame_result* d_result, void* scratch, uint64_t scratch_bytes,
                               void* stream, sb_error* err);
 /* Decode (read::FrameDecoder, src/read.rs:104-239) of a frame stream in device
- * memory. With d_chunk_offs/nchunks (the encoder's index; d_chunk_offs[nchunks]
- * = n) the chunk headers are parsed in parallel; without it (or when the index
- * does not describe a clean run of data chunks) one thread walks the headers in
- * stream order exactly like the reference's reader. Then one warp per chunk:
+ * memory. With d_chunk_offs/nchunks (the encoder's index, or the one
+ * sb_frame_index_device_ws builds; d_chunk_offs[nchunks] = n) the chunk headers
+ * are parsed in parallel. Without it the decoder first builds the index itself
+ * on the device (in its own scratch, no host synchronisation); when the stream is
+ * not a clean run of data chunks (skippable/padding chunks, a repeated
+ * identifier, ...) or an index does not describe it, one thread walks the
+ * headers in stream order exactly like the reference's reader. Then one warp per chunk:
  * raw decode (K2) or copy, masked CRC-32C of the produced bytes against the
  * header. d_result: first error in stream order + bytes produced before it.
  *   flags bit0: no stream identifier expected (a rank's fragment of a sharded stream)
@@ -182,6 +185,21 @@ int sb_frame_decode_device_ws(const uint8_t* d_in, uint64_t n, uint8_t* d_out, u
 int sb_frame_decode_device(const uint8_t* d_in, uint64_t n, uint8_t* d_out, uint64_t cap,
                            const uint64_t* d_chunk_offs, uint32_t nchunks, uint32_t flags,
                            sb_frame_result* result, void* stream, sb_error* err);
+
+/* Chunk index of a frame stream in device memory, built in parallel on the device:
+ * the offset of every chunk header in d_in[0..n) followed by n -- exactly the
+ * d_chunk_offs that sb_frame_decode_device_ws accepts (max_chunks + 1 entries).
+ * Only clean streams are indexed: the stream identifier (none when flags bit0,
+ * a fragment), then data chunks only, covering the stream exactly. *d_count
+ * (device) receives the number of chunks, or SB_FRAME_NOT_INDEXABLE for anything
+ * else (skippable or padding chunks, a repeated identifier, reserved chunk types,
+ * truncation, more than max_chunks chunks). Stream ordered, caller scratch of
+ * sb_frame_index_scratch_bytes(n, max_chunks) bytes, no allocation. Index a
+ * stream once to decode it many times, or to hand a rank a chunk range. */
+#define SB_FRAME_NOT_INDEXABLE 0xFFFFFFFFu
+uint64_t sb_frame_index_scratch_bytes(uint64_t n, uint32_t max_chunks);
+int sb_frame_index_device_ws(const uint8_t* d_in, uint64_t n, uint32_t flags, uint64_t* d_chunk_offs, uint32_t max_chunks,
+                             uint32_t* d_count, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
 
 /* ---- resources -------------------------------------------------------------
  * The host entry points keep grow-only per-device pools (device staging, pinned

@@ -4,9 +4,12 @@
 // frame stream that already sits in device memory; the per-chunk payload decode is K2 (k2_decompress.cuh) and the
 // checksum is K3's warp CRC, both run by the same warp while the chunk's output is still in L2.
 //
-//   k5_parse   (with a chunk index, e.g. the one the frame encoder emits): one thread per chunk validates the header,
-//              reads the checksum and the decompressed length. Anything unusual raises `need_serial`.
-//   k5_walk    (no index, or need_serial): one thread walks the chunk headers in stream order exactly like the
+//   k7         (no caller index): builds the chunk index of a clean stream in parallel (k7_frame_index.cuh) into
+//              `ooff`, or declines; its count stays on the device (`index_count`).
+//   k5_parse   (with a chunk index: the caller's, e.g. the one the frame encoder emits, or K7's): one thread per chunk
+//              validates the header, reads the checksum and the decompressed length. Anything unusual -- including a
+//              declined K7 index -- raises `need_serial`.
+//   k5_walk    (need_serial): one thread walks the chunk headers in stream order exactly like the
 //              reference's reader, including its quirk that decompress_len() sees the persistent source buffer
 //              (src/read.rs:216) -- ~1 us per chunk, since every header is a dependent global load.
 //   scan       output offset of every chunk (generic scan of k4_frame.cuh)
@@ -24,11 +27,13 @@ namespace sbk {
 static const uint32_t K5_MAX_CBLOCK = 76490;    // reference src/frame.rs:12 (MAX_COMPRESS_BLOCK_SIZE)
 
 struct FChunk { uint64_t body_off; uint32_t body_len; uint32_t dlen; uint32_t want_crc; uint32_t type; };
-struct DecodeCtl { uint32_t nchunks; uint32_t need_serial; uint64_t produced; sb_error walk_err; uint32_t go; uint32_t first_bad; };
+struct DecodeCtl { uint32_t nchunks; uint32_t need_serial; uint64_t produced; sb_error walk_err; uint32_t go; uint32_t first_bad;
+                   uint32_t index_count; };
 
 struct DecodePlan {
     const uint8_t* in; uint64_t n;             // frame stream (device)
     const uint64_t* index; uint32_t index_n;   // optional: offset of every chunk header; index[index_n] = n
+    const uint32_t* index_count;               // set: index_n is read here on the device (K7), SB_FRAME_NOT_INDEXABLE = none
     uint32_t fragment;                         // 1: no stream identifier expected (a rank's shard of a stream)
     FChunk* chunks; uint32_t cap_chunks;
     uint64_t* ooff;                            // cap_chunks + 1
@@ -59,18 +64,23 @@ SB_DEVICE uint32_t k5_varint(const uint8_t* p, uint32_t n, uint64_t* out) {
 SB_DEVICE void k5_parse_body(const DecodePlan& p) {
     const uint64_t i = (uint64_t)block_idx() * block_dim() + thread_idx();
     DecodeCtl* ctl = p.ctl;
+    const uint32_t index_n = p.index_count ? *p.index_count : p.index_n;
+    if (index_n == SB_FRAME_NOT_INDEXABLE) {                           // K7 declined: the walk decodes the stream
+        if (i == 0) { ctl->need_serial = 1; ctl->nchunks = 0; }
+        return;
+    }
     if (i == 0) {
-        bool ok = p.index_n <= p.cap_chunks && p.index[p.index_n] == p.n;
-        const uint64_t first = p.index_n ? p.index[0] : p.n;
+        bool ok = index_n <= p.cap_chunks && p.index[index_n] == p.n;
+        const uint64_t first = index_n ? p.index[0] : p.n;
         if (p.fragment) ok = ok && first == 0;
         else {
             ok = ok && first == 10 && p.n >= 10;
             if (ok) { const uint8_t id[10] = {0xFF, 6, 0, 0, 's', 'N', 'a', 'P', 'p', 'Y'}; for (int k = 0; k < 10; k++) ok = ok && p.in[k] == id[k]; }
         }
         if (!ok) ctl->need_serial = 1;
-        ctl->nchunks = p.index_n <= p.cap_chunks ? p.index_n : 0;
+        ctl->nchunks = index_n <= p.cap_chunks ? index_n : 0;
     }
-    if (i >= p.index_n || i >= p.cap_chunks) return;
+    if (i >= index_n || i >= p.cap_chunks) return;
     const uint64_t at = p.index[i], next = p.index[i + 1];
     bool ok = at + 8 <= p.n && next > at && next <= p.n;
     FChunk c;

@@ -19,6 +19,7 @@
 #include "k3_crc32c.cuh"
 #include "k4_frame.cuh"
 #include "k5_frame_decode.cuh"
+#include "k7_frame_index.cuh"
 
 namespace {
 
@@ -46,6 +47,9 @@ __global__ void __launch_bounds__(1024) k5_scan_tiles_kernel(sbk::DecodePlan p) 
 __global__ void __launch_bounds__(128) k5_decode_kernel(sbk::DecodePlan p) { sbk::k5_decode_body(p); }
 __global__ void __launch_bounds__(32) k5_finish_kernel(sbk::DecodePlan p) { sbk::k5_finish_body(p); }
 __global__ void __launch_bounds__(256) k6_generate_kernel(sbk::GenPlan g) { sbk::k6_generate_body(g); }
+__global__ void __launch_bounds__(128) k7_survivors_kernel(sbk::IndexPlan p) { sbk::k7_survivors_body(p); }
+__global__ void __launch_bounds__(sbk::K7_STITCH_THREADS) k7_stitch_kernel(sbk::IndexPlan p) { sbk::k7_stitch_body(p); }
+__global__ void __launch_bounds__(128) k7_emit_kernel(sbk::IndexPlan p) { sbk::k7_emit_body(p); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -360,12 +364,41 @@ sbk::DecodePlan make_decode_plan(const uint8_t* d_in, uint64_t n, uint8_t* d_out
     p.in = d_in; p.n = n; p.index = d_index; p.index_n = d_index ? index_n : 0; p.fragment = fragment ? 1u : 0u;
     p.chunks = w.chunks; p.cap_chunks = max_chunks; p.ooff = w.ooff; p.tiles = w.tiles; p.statuses = w.statuses; p.ctl = w.ctl;
     p.out = d_out; p.cap = cap; p.result = d_result;
+    if (!d_index) { p.index = w.ooff; p.index_count = &w.ctl->index_count; }   // K7 builds the index there
     return p;
 }
+
+// SNAPB200_K7_SEG = K7 segment length in bytes (floor 128 KiB; the survivor table may force it larger)
+uint64_t k7_want_seg() {
+    static const long long env = getenv("SNAPB200_K7_SEG") ? atoll(getenv("SNAPB200_K7_SEG")) : 0;
+    return env > 0 ? (uint64_t)env : sbk::K7_SEG_DEFAULT;
+}
+int launch_k7(Ctx& c, const sbk::IndexPlan& p, cudaStream_t st, sb_error* err) {
+    k7_survivors_kernel<<<p.nseg ? (p.nseg + 3) / 4 : 1, 128, 0, st>>>(p);
+    k7_stitch_kernel<<<1, sbk::K7_STITCH_THREADS, sbk::K7_STITCH_SMEM, st>>>(p);
+    k7_emit_kernel<<<p.nseg ? (p.nseg + 127) / 128 : 1, 128, 0, st>>>(p);
+    g_launches += 3;
+    CK(cudaGetLastError());
+    return 0;
+}
+// caller scratch of sb_frame_index_device_ws: survivor table + per-segment words, sized for the default segment length
+uint64_t index_ws_segs(uint64_t n) { return n / sbk::K7_SEG_DEFAULT + 2; }
+uint64_t index_ws_bytes(uint64_t n) {
+    return align_up(index_ws_segs(n) * sizeof(sbk::K7Seg), 256) + align_up(index_ws_segs(n) * 12, 256) + 256;
+}
+
 // phase 1: chunk table + output offsets (ctl->produced, ctl->go valid afterwards)
 int decode_index_phase(Ctx& c, const sbk::DecodePlan& p, cudaStream_t st, sb_error* err) {
     CK(cudaMemsetAsync(p.ctl, 0, sizeof(sbk::DecodeCtl), st));
-    if (p.index) { k5_parse_kernel<<<p.index_n ? (p.index_n + 255) / 256 : 1, 256, 0, st>>>(p); g_launches++; }
+    if (p.index_count) {
+        const int rc = launch_k7(c, sbk::k7_plan_for_decode(p, k7_want_seg()), st, err);
+        if (rc) return rc;
+    }
+    if (p.index) {
+        const uint64_t threads = p.index_count ? p.cap_chunks : p.index_n;   // K7's count is only known on the device
+        k5_parse_kernel<<<threads ? (unsigned)((threads + 255) / 256) : 1, 256, 0, st>>>(p);
+        g_launches++;
+    }
     k5_walk_kernel<<<1, 32, 0, st>>>(p);
     const unsigned ntiles = (p.cap_chunks + sbk::K4_TILE - 1) / sbk::K4_TILE;
     k5_scan_local_kernel<<<ntiles ? ntiles : 1, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(p);
@@ -974,7 +1007,8 @@ int sb_frame_encode_ex(const uint8_t* in, size_t n, uint8_t* out, size_t cap, si
 
 // Device-resident frame decode, stream ordered, caller-provided scratch (reference src/read.rs:104-239).
 //   d_chunk_offs/nchunks: optional index (offset of every chunk header, d_chunk_offs[nchunks] = n) -- the array
-//     sb_frame_encode_device_ws emits; without it one thread walks the headers (~1 us per chunk).
+//     sb_frame_encode_device_ws emits; without it K7 builds one in the decode scratch, and only a stream K7 declines
+//     is walked by one thread (~1 us per chunk).
 //   flags bit0: the stream has no identifier (a rank's fragment of a sharded stream).
 int sb_frame_decode_device_ws(const uint8_t* d_in, uint64_t n, uint8_t* d_out, uint64_t cap,
                               const uint64_t* d_chunk_offs, uint32_t nchunks, uint32_t flags,
@@ -996,9 +1030,10 @@ int sb_frame_decode_device_ws(const uint8_t* d_in, uint64_t n, uint8_t* d_out, u
         sbk::DecodeCtl h;
         cudaStreamSynchronize(st);
         cudaMemcpy(&h, p.ctl, sizeof h, cudaMemcpyDeviceToHost);
-        fprintf(stderr, "[frame decode] n=%llu index_n=%u fragment=%u cap_chunks=%u -> nchunks=%u need_serial=%u produced=%llu walk_err=%u(%llu,%llu) go=%u first_bad=%u\n",
-                (unsigned long long)n, p.index_n, p.fragment, p.cap_chunks, h.nchunks, h.need_serial, (unsigned long long)h.produced,
-                h.walk_err.code, (unsigned long long)h.walk_err.a, (unsigned long long)h.walk_err.b, h.go, h.first_bad);
+        fprintf(stderr, "[frame decode] n=%llu index_n=%u fragment=%u cap_chunks=%u k7=%u k7_count=%u -> nchunks=%u need_serial=%u produced=%llu walk_err=%u(%llu,%llu) go=%u first_bad=%u\n",
+                (unsigned long long)n, p.index_n, p.fragment, p.cap_chunks, p.index_count ? 1u : 0u, h.index_count, h.nchunks,
+                h.need_serial, (unsigned long long)h.produced, h.walk_err.code, (unsigned long long)h.walk_err.a,
+                (unsigned long long)h.walk_err.b, h.go, h.first_bad);
     }
     ok(err);
     return 0;
@@ -1036,8 +1071,30 @@ int sb_frame_decode_device(const uint8_t* d_in, uint64_t n, uint8_t* d_out, uint
     return 0;
 }
 
+// Chunk index alone (K7). max_chunks does not change the size: the table holds one record per segment of the stream.
+uint64_t sb_frame_index_scratch_bytes(uint64_t n, uint32_t max_chunks) { (void)max_chunks; return index_ws_bytes(n); }
+
+int sb_frame_index_device_ws(const uint8_t* d_in, uint64_t n, uint32_t flags, uint64_t* d_chunk_offs, uint32_t max_chunks,
+                             uint32_t* d_count, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if ((!d_in && n) || !d_chunk_offs || !d_count || !scratch) return fail(err, SB_E_INVALID);
+    if (scratch_bytes < index_ws_bytes(n)) return fail(err, SB_BUFFER_TOO_SMALL, scratch_bytes, index_ws_bytes(n));
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    const uint64_t segs = index_ws_segs(n);
+    uint8_t* q = (uint8_t*)align_up((size_t)scratch, 256);
+    sbk::K7Seg* table = (sbk::K7Seg*)q;
+    uint32_t* meta = (uint32_t*)(q + align_up(segs * sizeof(sbk::K7Seg), 256));
+    // a table sized for the default segment length holds no more segments than that (k7_seg_len grows shorter ones)
+    const sbk::IndexPlan p = sbk::k7_make_plan(d_in, n, flags & 1u, max_chunks, k7_want_seg(), table, segs, meta, d_chunk_offs, d_count);
+    rc = launch_k7(*c, p, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
 // read::FrameDecoder + read_to_end over host memory (reference src/read.rs:104-239): the stream is uploaded once
-// and decoded by the device path above (header walk, K2, checksum); the first failure IN STREAM ORDER is reported
+// and decoded by the device path above (K7 index or header walk, K2, checksum); the first failure IN STREAM ORDER is reported
 // and the bytes produced before it are returned, like a reader that fails on its n-th read.
 int sb_frame_decode(const uint8_t* in, size_t n, uint8_t* out, size_t cap, size_t* out_n, sb_error* err) {
     if ((!in && n) || !out_n) return fail(err, SB_E_INVALID);
