@@ -76,7 +76,9 @@ SB_DEVICE uint32_t k3_slice(const uint32_t* tab, uint32_t st, const uint8_t* p, 
 // masked CRC-32C of [p, p+n) computed by the calling warp; result in all lanes
 SB_DEVICE uint32_t k3_warp_crc32c_masked(const uint32_t* tab, const uint8_t* p, uint32_t n) {
     const unsigned lane = lane_id();
-    uint32_t sl = ((n + 31) / 32 + 3) & ~3u;       // slice length, multiple of 4
+    // slice length ceil(n/32) rounded up to a multiple of 4; as ((n - 1) >> 5) + 1 it cannot wrap near 2^32 like n + 31
+    // (n = 0 gives a huge slice, but every slice is clipped to [0, n) and stays empty)
+    uint32_t sl = (((n - 1) >> 5) + 4) & ~3u;
     if (sl < 64) sl = 64;
     uint64_t b0 = (uint64_t)lane * sl, b1 = b0 + sl;
     if (b0 > n) b0 = n;
@@ -126,7 +128,7 @@ SB_DEVICE uint32_t k3_slice1(const uint32_t* tab, uint32_t st, const uint8_t* p,
 // masked CRC-32C of [p, p+n) by the calling warp with the byte table; result in all lanes
 SB_DEVICE uint32_t k3_warp_crc32c_masked1(const uint32_t* tab, const uint8_t* p, uint32_t n) {
     const unsigned lane = lane_id();
-    uint32_t sl = ((n + 31) / 32 + 15) & ~15u;     // slice length, multiple of 16
+    uint32_t sl = (((n - 1) >> 5) + 16) & ~15u;    // ceil(n/32) rounded up to a multiple of 16, without wrapping (see k3_warp_crc32c_masked)
     if (sl < 64) sl = 64;
     uint64_t b0 = (uint64_t)lane * sl, b1 = b0 + sl;
     if (b0 > n) b0 = n;

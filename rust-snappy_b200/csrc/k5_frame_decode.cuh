@@ -233,7 +233,10 @@ SB_DEVICE void k5_finish_body(const DecodePlan& p) {
     const DecodeCtl* ctl = p.ctl;
     sb_frame_result r;
     r.nchunks = ctl->nchunks; r._pad = 0;
-    if (!ctl->go) { k5_set(&r.status, SB_BUFFER_TOO_SMALL, p.cap, ctl->produced); r.bytes = 0; }
+    // chunk table too small: the walk stopped early, so `produced` is only a lower bound -- report the table first, so
+    // that a caller retries with a larger one before it sizes the output
+    if (ctl->walk_err.code == SB_E_INVALID && ctl->walk_err.b == 1) { r.status = ctl->walk_err; r.bytes = 0; }
+    else if (!ctl->go) { k5_set(&r.status, SB_BUFFER_TOO_SMALL, p.cap, ctl->produced); r.bytes = 0; }
     else if (ctl->first_bad != 0xFFFFFFFFu) { r.status = p.statuses[ctl->first_bad]; r.bytes = p.ooff[ctl->first_bad]; }
     else { r.status = ctl->walk_err; r.bytes = ctl->produced; }
     *p.result = r;
