@@ -75,6 +75,20 @@ int sb_decompress_len(const uint8_t* in, size_t n, size_t* out_len, sb_error* er
  * variant and payload of the reference on corrupt input. */
 int sb_decompress(const uint8_t* in, size_t n, uint8_t* out, size_t cap, size_t* out_n, sb_error* err);
 
+/* Stream-ordered raw decode of one stream d_in[0..n) in device memory into d_out[0..cap), caller scratch of
+ * sb_decompress_scratch_bytes(n) bytes (sized from the compressed length alone), no allocation, no host
+ * synchronisation. The stream's 64 KB blocks are located on the device and decoded in parallel, one warp per block;
+ * a stream that is not split that way (copies reaching into an earlier block, elements across a block boundary,
+ * literals over 64 KB, corrupt or truncated data) is decoded by one warp exactly as before. *d_result (device):
+ * status = Ok or the reference's error, bytes = the decompressed length on Ok (0 otherwise), nchunks = blocks decoded
+ * in parallel (0 when the one-warp path ran). On error d_out beyond what was decoded is unspecified. n above
+ * 2^32 - 1, null pointers and scratch that is too small are SB_E_INVALID. sb_decompress takes this path for every
+ * stream whose header announces more than 65536 bytes. */
+uint64_t sb_decompress_scratch_bytes(uint64_t n);
+int sb_decompress_device_ws(const uint8_t* d_in, uint64_t n, uint8_t* d_out, uint64_t cap,
+                            sb_frame_result* d_result, void* scratch, uint64_t scratch_bytes,
+                            void* stream, sb_error* err);
+
 /* crc32::CheckSummer::crc32c_masked (src/crc32.rs:35-38), computed on device. */
 int sb_crc32c_masked(const uint8_t* in, size_t n, uint32_t* out, sb_error* err);
 

@@ -32,7 +32,8 @@ class SbBatch(C.Structure):
 
 # every symbol include/snapb200.h declares
 SYMBOLS = [
-    "sb_max_compress_len", "sb_compress", "sb_decompress_len", "sb_decompress", "sb_crc32c_masked",
+    "sb_max_compress_len", "sb_compress", "sb_decompress_len", "sb_decompress", "sb_decompress_scratch_bytes",
+    "sb_decompress_device_ws", "sb_crc32c_masked",
     "sb_compress_batch_host", "sb_decompress_batch_host", "sb_compress_batch_host_packed",
     "sb_compress_batch_device", "sb_decompress_batch_device", "sb_crc32c_masked_batch_device",
     "sb_frame_max_len", "sb_frame_encode", "sb_frame_encode_ex", "sb_frame_decode", "sb_frame_encode_device",
@@ -67,6 +68,9 @@ def lib():
     L.sb_compress.argtypes = [vp, sz, vp, sz, szp, ep]
     L.sb_decompress_len.argtypes = [vp, sz, szp, ep]
     L.sb_decompress.argtypes = [vp, sz, vp, sz, szp, ep]
+    L.sb_decompress_scratch_bytes.restype = C.c_uint64
+    L.sb_decompress_scratch_bytes.argtypes = [C.c_uint64]
+    L.sb_decompress_device_ws.argtypes = [vp, C.c_uint64, vp, C.c_uint64, vp, vp, C.c_uint64, vp, ep]
     L.sb_crc32c_masked.argtypes = [vp, sz, u32p, ep]
     L.sb_compress_batch_host.argtypes = [vp, vp, vp, vp, vp, vp, vp, sz, ep]
     L.sb_decompress_batch_host.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, sz, ep]

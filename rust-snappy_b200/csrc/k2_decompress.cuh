@@ -36,16 +36,24 @@ SB_DEVICE uint32_t k2_read_header(const uint8_t* in, uint32_t n, uint64_t* value
     return 0;
 }
 
-// Decode one raw stream with the calling warp. Returns the status code.
+// Decode one raw stream with the calling warp. Returns the status code. kHeader = false: `in` is the element sequence
+// of one block alone (no varint header) that must produce exactly `cap` bytes -- K8 (k8_raw_split.cuh) hands every
+// block of a split stream to its own warp this way, and the reference's checks are then made against the block's
+// bounds, which are stricter than the stream's.
+template <bool kHeader = true>
 SB_DEVICE uint32_t k2_decode_stream(const uint8_t* in, uint32_t n, uint8_t* dst, uint64_t cap,
                                     sb_error* st, uint32_t* out_len, uint32_t* elems) {
     const unsigned lane = lane_id();
-    if (n == 0) { if (lane == 0) set_status(st, SB_EMPTY, 0, 0, 0); return SB_EMPTY; }
-    uint64_t dn64 = 0;
-    const uint32_t hl = k2_read_header(in, n, &dn64);
-    if (hl == 0) { if (lane == 0) set_status(st, SB_HEADER, 0, 0, 0); return SB_HEADER; }
-    if (dn64 > kMaxInput) { if (lane == 0) set_status(st, SB_TOO_BIG, dn64, kMaxInput, 0); return SB_TOO_BIG; }
-    if (dn64 > cap) { if (lane == 0) set_status(st, SB_BUFFER_TOO_SMALL, cap, dn64, 0); return SB_BUFFER_TOO_SMALL; }
+    uint64_t dn64 = cap;
+    uint32_t hl = 0;
+    if constexpr (kHeader) {
+        if (n == 0) { if (lane == 0) set_status(st, SB_EMPTY, 0, 0, 0); return SB_EMPTY; }
+        dn64 = 0;
+        hl = k2_read_header(in, n, &dn64);
+        if (hl == 0) { if (lane == 0) set_status(st, SB_HEADER, 0, 0, 0); return SB_HEADER; }
+        if (dn64 > kMaxInput) { if (lane == 0) set_status(st, SB_TOO_BIG, dn64, kMaxInput, 0); return SB_TOO_BIG; }
+        if (dn64 > cap) { if (lane == 0) set_status(st, SB_BUFFER_TOO_SMALL, cap, dn64, 0); return SB_BUFFER_TOO_SMALL; }
+    }
 
     const uint8_t* src = in + hl;
     const uint8_t* in_end = in + n;
@@ -53,61 +61,7 @@ SB_DEVICE uint32_t k2_decode_stream(const uint8_t* in, uint32_t n, uint8_t* dst,
     uint32_t s = 0, d = 0;
 
     while (s < sn) {
-        // ---- fetch 40 bytes starting at the 4-byte-aligned address below src+s
-        const uintptr_t A = (uintptr_t)(src + s);
-        const unsigned mis = (unsigned)(A & 3u);
-        uint32_t word = 0;
-        if (lane < 10) {
-            const uint8_t* wp = (const uint8_t*)(A - mis) + 4 * lane;
-            if (wp >= in && wp + 4 <= in_end) {
-                word = *(const uint32_t*)wp;
-            } else {
-                for (int k = 0; k < 4; k++)
-                    if (wp + k >= in && wp + k < in_end) word |= (uint32_t)wp[k] << (8 * k);
-            }
-        }
-        const unsigned bi = mis + lane;
-        const uint32_t lo = shfl(word, bi >> 2), hi = shfl(word, (bi >> 2) + 1);
-        const unsigned sh = (bi & 3u) * 8;
-        const uint32_t tag = funnel_r(lo, hi, sh) & 0xFFu;          // byte at s+lane
-        const uint32_t next4 = sh == 24 ? hi : funnel_r(lo, hi, sh + 8);  // 4 bytes after it
-        const uint32_t rem = sn - s;                                 // bytes left from window start
-        const bool valid = lane < rem;
-
-        // ---- speculative element decode (tag layout: build.rs:40-67)
-        const unsigned kind = tag & 3u;
-        unsigned hdr;       // tag byte + trailer bytes
-        uint64_t len;       // output bytes produced
-        uint32_t off = 0;
-        if (kind == 0) {
-            const unsigned L = tag >> 2;
-            if (L < 60) { hdr = 1; len = L + 1; }
-            else {
-                const unsigned nb = L - 59;
-                hdr = 1 + nb;
-                len = (uint64_t)(nb == 4 ? next4 : (next4 & ((1u << (8 * nb)) - 1))) + 1;
-            }
-        } else if (kind == 1) {
-            hdr = 2; len = 4 + ((tag >> 2) & 7u); off = ((tag >> 5) << 8) | (next4 & 0xFFu);
-        } else if (kind == 2) {
-            hdr = 3; len = 1 + (tag >> 2); off = next4 & 0xFFFFu;
-        } else {
-            hdr = 5; len = 1 + (tag >> 2); off = next4;
-        }
-        // a literal whose payload does not end inside this window ("spill") closes the window
-        const bool spill = valid && kind == 0 && (uint64_t)lane + hdr + len > 32;
-        uint32_t E = !valid ? 64u : spill ? 64u : (uint32_t)(lane + hdr + (kind == 0 ? (uint32_t)len : 0u));
-
-        // ---- true element starts: pointer doubling from every lane, read lane 0
-        // every element occupies at least 2 compressed bytes (tag + payload/offset byte), so the chain
-        // from lane 0 has at most 16 nodes inside the window: four doubling rounds always suffice
-        uint32_t M = 1u << lane;
-#pragma unroll
-        for (int r = 0; r < 4; r++) {
-            const uint32_t M2 = shfl(M, E & 31u), E2 = shfl(E, E & 31u);
-            if (E < 32) { M |= M2; E = E2; }
-        }
-        M = shfl(M, 0);
+#include "k2_window.inc"
         const bool is_start = ((M >> lane) & 1u) && valid;
         const unsigned last = 31 - clz(M);
 

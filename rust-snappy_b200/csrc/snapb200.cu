@@ -20,6 +20,7 @@
 #include "k4_frame.cuh"
 #include "k5_frame_decode.cuh"
 #include "k7_frame_index.cuh"
+#include "k8_raw_split.cuh"
 
 namespace {
 
@@ -50,6 +51,16 @@ __global__ void __launch_bounds__(256) k6_generate_kernel(sbk::GenPlan g) { sbk:
 __global__ void __launch_bounds__(128) k7_survivors_kernel(sbk::IndexPlan p) { sbk::k7_survivors_body(p); }
 __global__ void __launch_bounds__(sbk::K7_STITCH_THREADS) k7_stitch_kernel(sbk::IndexPlan p) { sbk::k7_stitch_body(p); }
 __global__ void __launch_bounds__(128) k7_emit_kernel(sbk::IndexPlan p) { sbk::k7_emit_body(p); }
+__global__ void __launch_bounds__(32) k8_header_kernel(sbk::RawPlan p) { sbk::k8_header_body(p); }
+__global__ void __launch_bounds__(128) k8_chains_kernel(sbk::RawPlan p) { sbk::k8_chains_body(p); }
+__global__ void __launch_bounds__(128) k8_merge_kernel(sbk::RawPlan p) { sbk::k8_merge_body(p); }
+__global__ void __launch_bounds__(sbk::K8_STITCH_THREADS) k8_stitch_kernel(sbk::RawPlan p) { sbk::k8_stitch_body(p); }
+__global__ void __launch_bounds__(128) k8_counts_kernel(sbk::RawPlan p) { sbk::k8_counts_body(p); }
+__global__ void __launch_bounds__(1024) k8_scan_local_kernel(sbk::RawPlan p) { sbk::k8_scan_local_body(p); }
+__global__ void __launch_bounds__(1024) k8_scan_tiles_kernel(sbk::RawPlan p) { sbk::k8_scan_tiles_body(p); }
+__global__ void __launch_bounds__(128) k8_cuts_kernel(sbk::RawPlan p) { sbk::k8_cuts_body(p); }
+__global__ void __launch_bounds__(128) k8_blocks_kernel(sbk::RawPlan p) { sbk::k8_blocks_body(p); }
+__global__ void __launch_bounds__(32) k8_fallback_kernel(sbk::RawPlan p) { sbk::k8_fallback_body(p); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -416,6 +427,63 @@ int decode_payload_phase(Ctx& c, const sbk::DecodePlan& p, cudaStream_t st, sb_e
     return 0;
 }
 
+// ---- raw stream decode (K8 split + block decode, or the one-warp fallback)
+// scratch: control record, start bitmap, per-segment records for segments of at least K8_SEG_MIN, the cut table
+uint64_t raw_ws_bytes(uint64_t n) {
+    const uint64_t segs = sbk::k8_max_segs(n);
+    return 256 + align_up(((n >> 5) + 2) * 4, 256) + 4 * align_up(segs * 8, 256) + align_up(segs * 4, 256) +
+           align_up((segs + 1) * 8, 256) + align_up((segs / sbk::K4_TILE + 3) * 8, 256) +
+           align_up(((uint64_t)sbk::K8_MAX_BLOCKS + 1) * 4, 256) + 256;
+}
+sbk::RawPlan make_raw_plan(const uint8_t* d_in, uint64_t n, uint8_t* d_out, uint64_t cap, sb_frame_result* d_result,
+                           void* scratch, uint64_t want_seg) {
+    const uint64_t segs = sbk::k8_max_segs(n);
+    uint8_t* q = (uint8_t*)align_up((size_t)scratch, 256);
+    sbk::RawPlan p;
+    memset(&p, 0, sizeof p);
+    p.in = d_in; p.n = n; p.out = d_out; p.cap = cap; p.result = d_result;
+    p.seg = sbk::k8_seg_len(want_seg);
+    p.nseg = (uint32_t)((n + p.seg - 1) / p.seg);
+    p.ctl = (sbk::RawCtl*)q; q += 256;
+    p.marks = (uint32_t*)q; q += align_up(((n >> 5) + 2) * 4, 256);
+    p.X = (uint64_t*)q; q += align_up(segs * 8, 256);
+    p.Y = (uint64_t*)q; q += align_up(segs * 8, 256);
+    p.ent = (uint64_t*)q; q += align_up(segs * 8, 256);
+    p.ext = (uint64_t*)q; q += align_up(segs * 8, 256);
+    p.cnt = (uint32_t*)q; q += align_up(segs * 4, 256);
+    p.offs = (uint64_t*)q; q += align_up((segs + 1) * 8, 256);
+    p.tiles = (uint64_t*)q; q += align_up((segs / sbk::K4_TILE + 3) * 8, 256);
+    p.cut = (uint32_t*)q;
+    return p;
+}
+// SNAPB200_K8_SEG = K8 segment length in compressed bytes (floor 128 KiB); read on every call
+uint64_t k8_want_seg() {
+    const char* v = getenv("SNAPB200_K8_SEG");
+    return v && atoll(v) > 0 ? (uint64_t)atoll(v) : 0;
+}
+int launch_raw_decode(Ctx& c, const sbk::RawPlan& p, cudaStream_t st, sb_error* err) {
+    const unsigned segw = p.nseg ? (p.nseg + 3) / 4 : 1;
+    CK(cudaMemsetAsync(p.marks, 0, ((p.n >> 5) + 2) * 4, st));
+    k8_header_kernel<<<1, 32, 0, st>>>(p);
+    k8_chains_kernel<<<segw, 128, 0, st>>>(p);
+    k8_merge_kernel<<<segw, 128, 0, st>>>(p);
+    k8_stitch_kernel<<<1, sbk::K8_STITCH_THREADS, sbk::K8_STITCH_THREADS * 16 + 16, st>>>(p);
+    k8_counts_kernel<<<segw, 128, 0, st>>>(p);
+    const unsigned ntiles = (p.nseg + sbk::K4_TILE - 1) / sbk::K4_TILE;
+    k8_scan_local_kernel<<<ntiles ? ntiles : 1, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(p);
+    k8_scan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(p);
+    k8_cuts_kernel<<<segw, 128, 0, st>>>(p);
+    // blocks: at most ceil(min(cap, 2^32 - 1) / 65536); the true count is on the device
+    const uint64_t ocap = p.cap < SB_MAX_INPUT ? p.cap : SB_MAX_INPUT;
+    const uint64_t bgrid = ((ocap + 65535) / 65536 + 3) / 4;
+    const unsigned grid = bgrid == 0 ? 1 : bgrid < (uint64_t)(16 * c.sms) ? (unsigned)bgrid : (unsigned)(16 * c.sms);
+    k8_blocks_kernel<<<grid, 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(p);
+    k8_fallback_kernel<<<1, 32, sbk::K2_SMEM_PER_WARP, st>>>(p);
+    g_launches += 10;
+    CK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 // =========================================================================
@@ -501,6 +569,20 @@ int sb_reserve(size_t wave_units, size_t wave_in_bytes, size_t wave_out_bytes, s
 
 uint64_t sb_frame_encode_scratch_bytes(uint64_t n) { return encode_ws_bytes(n); }
 uint64_t sb_frame_decode_scratch_bytes(uint32_t max_chunks) { return decode_ws_bytes(max_chunks); }
+uint64_t sb_decompress_scratch_bytes(uint64_t n) { return raw_ws_bytes(n); }
+
+int sb_decompress_device_ws(const uint8_t* d_in, uint64_t n, uint8_t* d_out, uint64_t cap, sb_frame_result* d_result,
+                            void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if ((!d_in && n) || (!d_out && cap) || !d_result || !scratch || n > SB_MAX_INPUT) return fail(err, SB_E_INVALID);
+    if (scratch_bytes < raw_ws_bytes(n)) return fail(err, SB_E_INVALID, scratch_bytes, raw_ws_bytes(n));
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_raw_decode(*c, make_raw_plan(d_in, n, d_out, cap, d_result, scratch, k8_want_seg()), (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
 
 int sb_compress(const uint8_t* in, size_t n, uint8_t* out, size_t cap, size_t* out_n, sb_error* err) {
     if ((!in && n) || !out || !out_n) return fail(err, SB_E_INVALID);
@@ -562,6 +644,25 @@ int sb_decompress(const uint8_t* in, size_t n, uint8_t* out, size_t cap, size_t*
     CK(l.status[0].need(sizeof(sb_error) + 16));
     rc = need_pinned(l, 4, 4096, err); if (rc) return rc;
     CK(cudaMemcpyAsync(l.in[0].p, in, n, cudaMemcpyHostToDevice, l.s_compute));
+    if (dcap > SB_MAX_BLOCK) {
+        // more than one block: K8 splits the stream and decodes its blocks in parallel (or declines, and one warp
+        // decodes it as below)
+        CK(l.ws[0].need(raw_ws_bytes(n) + sizeof(sb_frame_result) + 256));
+        sb_frame_result* d_res = (sb_frame_result*)((uint8_t*)l.ws[0].p + align_up(raw_ws_bytes(n), 256));
+        const uint64_t dev_cap = cap > SB_MAX_INPUT ? SB_MAX_INPUT : cap;
+        rc = launch_raw_decode(*c, make_raw_plan(l.in[0].as<uint8_t>(), n, l.compact[0].as<uint8_t>(), dev_cap, d_res, l.ws[0].p,
+                                                 k8_want_seg()), l.s_compute, err);
+        if (rc) return rc;
+        sb_frame_result* fr = (sb_frame_result*)l.pinned[4];
+        CK(cudaMemcpyAsync(fr, d_res, sizeof *fr, cudaMemcpyDeviceToHost, l.s_compute));
+        CK(cudaStreamSynchronize(l.s_compute));
+        if (fr->status.code) { if (err) *err = fr->status; return (int)fr->status.code; }
+        const uint64_t got = fr->bytes;
+        if (got) CK(cudaMemcpy(out, l.compact[0].p, got, cudaMemcpyDeviceToHost));
+        *out_n = (size_t)got;
+        ok(err);
+        return 0;
+    }
     sb_batch b;
     memset(&b, 0, sizeof b);
     b.in_base = l.in[0].as<uint8_t>(); b.in_len_uniform = (uint32_t)n;
