@@ -96,7 +96,8 @@ int sb_crc32c_masked(const uint8_t* in, size_t n, uint32_t* out, sb_error* err);
  * What a Rust caller holding many buffers (or the frame writers below) uses:
  * one call, pinned staging + H2D/D2H pipelined against the kernels inside.
  * Unit i reads in_base[in_offs[i] .. +in_lens[i]) and writes out_base[out_offs[i] ..];
- * out capacity per unit is out_caps[i]. statuses may be NULL for compress. */
+ * out capacity per unit is out_caps[i]. statuses may be NULL for compress. A decode wave holding a unit whose
+ * header announces more than 65536 bytes runs sb_decompress_batch_device_ws's block-parallel path. */
 int sb_compress_batch_host(const uint8_t* in_base, const uint64_t* in_offs, const uint32_t* in_lens,
                            uint8_t* out_base, const uint64_t* out_offs, const uint32_t* out_caps,
                            uint32_t* out_lens, size_t count, sb_error* err);
@@ -140,6 +141,21 @@ typedef struct sb_batch {
 int sb_compress_batch_device(const sb_batch* batch, void* stream, sb_error* err);
 /* Each unit is one raw stream; statuses[i] carries the reference's error. */
 int sb_decompress_batch_device(const sb_batch* batch, void* stream, sb_error* err);
+/* The same per-unit results as sb_decompress_batch_device (bytes, out_lens[i], statuses[i] with the reference's
+ * variant and payload; the same addressing), but every unit whose header announces more than 65536 bytes is split
+ * into its 64 KB blocks as sb_decompress_device_ws splits one stream, and the blocks of all units are decoded side by
+ * side in one grid. Units with at most one block, and units the split declines (a bad header or one over out_caps[i],
+ * a header announcing more output than the compressed length can encode, copies into an earlier block, elements
+ * across a block boundary, literals over 64 KB, corrupt or truncated data), are decoded by one warp exactly as before.
+ *   in_bytes: the caller's upper bound on the sum of the units' in_lens (which may live on the device); the scratch,
+ *     sb_decompress_batch_scratch_bytes(count, in_bytes) bytes, depends on nothing else. Bounds above 2^36 count as
+ *     2^36. When the lengths sum to more than in_bytes, no unit is split: results stay exact.
+ *   d_unit_blocks: optional (device, count entries): blocks decoded in parallel for unit i, 0 when one warp decoded it.
+ * Stream ordered, no allocation, no host synchronisation. out_lens is required. Null pointers, count >= 2^31 and
+ * scratch that is too small are SB_E_INVALID with nothing launched; count == 0 does nothing. */
+uint64_t sb_decompress_batch_scratch_bytes(uint32_t count, uint64_t in_bytes);
+int sb_decompress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t* d_unit_blocks,
+                                  void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
 /* Masked CRC-32C of each unit (frame chunks): out_lens[i] receives the CRC. */
 int sb_crc32c_masked_batch_device(const sb_batch* batch, void* stream, sb_error* err);
 

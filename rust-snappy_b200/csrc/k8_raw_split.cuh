@@ -192,23 +192,32 @@ SB_DEVICE void k8_header_body(const RawPlan& p) {
     *p.ctl = c;
 }
 
-SB_DEVICE void k8_chains_body(const RawPlan& p) {
-    const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
-    if (k >= p.nseg || k8_declined(p)) return;
+// The per-segment steps below take segment k (< p.nseg) of a stream that is not declined (k8_cuts_seg checks that
+// itself). The single-stream kernels give one warp per segment of p; the batch kernels (k8b_*) one warp per segment of
+// any unit's view.
+SB_DEVICE void k8_chains_seg(const RawPlan& p, uint64_t k) {
     const uint64_t b = k * p.seg, lim = b + p.seg < p.n ? b + p.seg : p.n;
     const uint64_t start = k ? b : p.ctl->hl;
     uint64_t out;
     const uint64_t x = start < lim ? k8_walk<true, false>(p, start, lim, 0, 0, &out) : start;
     if (lane_id() == 0) p.X[k] = x;
 }
-
-SB_DEVICE void k8_merge_body(const RawPlan& p) {
+SB_DEVICE void k8_chains_body(const RawPlan& p) {
     const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
-    if (k == 0 || k >= p.nseg || k8_declined(p)) return;
+    if (k >= p.nseg || k8_declined(p)) return;
+    k8_chains_seg(p, k);
+}
+
+SB_DEVICE void k8_merge_seg(const RawPlan& p, uint64_t k) {                  // k >= 1
     const uint64_t e = p.X[k - 1], lim = (k + 1) * p.seg < p.n ? (k + 1) * p.seg : p.n;
     uint64_t out;
     const uint64_t x = e < lim ? k8_walk<false, false, true>(p, e, lim, 0, 0, &out) : e;
     if (lane_id() == 0) p.Y[k] = x == K8_MET ? p.X[k] : x;
+}
+SB_DEVICE void k8_merge_body(const RawPlan& p) {
+    const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
+    if (k == 0 || k >= p.nseg || k8_declined(p)) return;
+    k8_merge_seg(p, k);
 }
 
 SB_DEVICE void k8_stitch_body(const RawPlan& p) {
@@ -242,13 +251,16 @@ SB_DEVICE void k8_stitch_body(const RawPlan& p) {
     if (t == 0 && (!sOk[0] || e != p.n)) p.ctl->decline = 1;
 }
 
-SB_DEVICE void k8_counts_body(const RawPlan& p) {
-    const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
-    if (k >= p.nseg || k8_declined(p)) return;
+SB_DEVICE void k8_counts_seg(const RawPlan& p, uint64_t k) {
     const uint64_t e = p.ent[k], x = p.ext[k];
     uint64_t out = 0;
     if (e < x) k8_walk<false, false>(p, e, x, 0, 0, &out);
     if (lane_id() == 0) p.cnt[k] = (uint32_t)out;
+}
+SB_DEVICE void k8_counts_body(const RawPlan& p) {
+    const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
+    if (k >= p.nseg || k8_declined(p)) return;
+    k8_counts_seg(p, k);
 }
 SB_DEVICE void k8_scan_local_body(const RawPlan& p) {
     const uint32_t* cnt = p.cnt;
@@ -257,21 +269,36 @@ SB_DEVICE void k8_scan_local_body(const RawPlan& p) {
 }
 SB_DEVICE void k8_scan_tiles_body(const RawPlan& p) { scan_tiles_body(p.nseg, 0, p.tiles); }
 
-SB_DEVICE void k8_cuts_body(const RawPlan& p) {
-    const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
+// total(): output bytes of the stream's segments (checked against dn by segment 0); obase(): output position of the
+// element at ent[k]. Both are evaluated only where they are needed.
+template <class Total, class Obase>
+SB_DEVICE void k8_cuts_seg(const RawPlan& p, uint64_t k, Total total, Obase obase) {
     RawCtl* ctl = p.ctl;
-    if (k >= p.nseg || k8_declined(p)) return;
+    if (k8_declined(p)) return;
     const uint64_t dn = ctl->dn;
     if (k == 0 && lane_id() == 0) {
-        if (p.tiles[(p.nseg + K4_TILE - 1) / K4_TILE] != dn) ctl->decline = 1;
+        if (total() != dn) ctl->decline = 1;
         p.cut[ctl->nblk] = (uint32_t)p.n;
     }
     const uint64_t e = p.ent[k], x = p.ext[k];
     uint64_t out;
-    if (e < x && k8_walk<false, true>(p, e, x, p.tiles[k / K4_TILE] + p.offs[k], dn, &out) == K8_BAD && lane_id() == 0)
+    if (e < x && k8_walk<false, true>(p, e, x, obase(), dn, &out) == K8_BAD && lane_id() == 0)
         ctl->decline = 1;
 }
+SB_DEVICE void k8_cuts_body(const RawPlan& p) {
+    const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
+    if (k >= p.nseg) return;
+    k8_cuts_seg(p, k, [&] { return p.tiles[(p.nseg + K4_TILE - 1) / K4_TILE]; },
+                [&] { return p.tiles[k / K4_TILE] + p.offs[k]; });
+}
 
+// block j of a split stream (dn: its decompressed length), decoded alone by the calling warp
+SB_DEVICE void k8_block(const RawPlan& p, uint64_t j, uint64_t dn, uint32_t* elems) {
+    const uint32_t a = p.cut[j], b = p.cut[j + 1];
+    const uint64_t want = dn - (j << 16) < 65536 ? dn - (j << 16) : 65536;
+    const uint32_t code = k2_decode_stream<false>(p.in + a, b - a, p.out + (j << 16), want, nullptr, nullptr, elems);
+    if (code != SB_OK && lane_id() == 0) p.ctl->decline = 1;
+}
 SB_DEVICE void k8_blocks_body(const RawPlan& p) {
     RawCtl* ctl = p.ctl;
     if (k8_declined(p)) return;
@@ -280,12 +307,7 @@ SB_DEVICE void k8_blocks_body(const RawPlan& p) {
     const uint64_t dn = ctl->dn;
     const unsigned wpb = block_dim() >> 5;
     const uint64_t nwarps = (uint64_t)grid_dim() * wpb;
-    for (uint64_t j = (uint64_t)block_idx() * wpb + warp_id(); j < nblk; j += nwarps) {
-        const uint32_t a = p.cut[j], b = p.cut[j + 1];
-        const uint64_t want = dn - (j << 16) < 65536 ? dn - (j << 16) : 65536;
-        const uint32_t code = k2_decode_stream<false>(p.in + a, b - a, p.out + (j << 16), want, nullptr, nullptr, elems);
-        if (code != SB_OK && lane_id() == 0) ctl->decline = 1;
-    }
+    for (uint64_t j = (uint64_t)block_idx() * wpb + warp_id(); j < nblk; j += nwarps) k8_block(p, j, dn, elems);
 }
 
 SB_DEVICE void k8_fallback_body(const RawPlan& p) {
@@ -301,6 +323,253 @@ SB_DEVICE void k8_fallback_body(const RawPlan& p) {
     const uint32_t code = k2_decode_stream(p.in, (uint32_t)p.n, p.out, p.cap, &r->status, &ctl->out_len, (uint32_t*)smem());
     syncwarp();
     if (lane_id() == 0) { r->bytes = code == SB_OK ? ctl->out_len : 0; r->nchunks = 0; r->_pad = 0; }
+}
+
+
+// ---------------------------------------------------------------------------------------------------------- K8 batch
+// K8 over a batch of raw streams (sb_decompress_batch_device_ws). Every unit whose header announces more than 65,536
+// bytes is split and its blocks decoded as above; the per-segment steps run on an ordinary RawPlan *view* of the unit
+// (its own input, output, control record and slices of the shared arrays), so the batch adds only the unit dimension.
+//   k8b_plan        thread per unit: the split verdict (RawCtl per unit) and three per-unit counts -- segments, blocks,
+//                   mark words -- scanned by K4's two-level scan (k8b_plan_tiles finishes it); Σ in_lens -> bctl.
+//   k8b_chains, k8b_merge, k8b_counts, k8b_cuts   warp per segment of the global segment list: binary search for
+//                   (unit, local segment), then the single-stream step on the unit's view.
+//   k8b_stitch      CTA per split unit: k8_stitch_body on its view.
+//   k8b_scan_*      K4's scan over the global segment list's output counts; a segment's output base is the scan
+//                   value minus the value at its unit's first segment.
+//   k8b_blocks      warp per block of the global block list.
+//   k8b_finish      warp per unit, always: split units get Ok, dn and their block count; every other unit (never split,
+//                   or declined anywhere above) is decoded by k2_decode_stream exactly as k2_decompress_body does.
+// A unit is split only when it has more than one block, fits its output, and its header announces no more output than
+// its body can encode (64 bytes per 3-byte copy-2 is the densest element). That bounds the blocks by the compressed
+// bytes, so every slice is sized from the caller's bound `in_bytes` on Σ in_lens; when the lengths on the device sum
+// to more than that, nothing is split and every unit takes the one-warp path.
+static const uint64_t K8B_MAX_IN_BYTES = 1ull << 36;   // larger bounds are clamped: 2^36 / 32 mark words per tile fit u32
+static const uint32_t K8B_MAX_COUNT = 1u << 31;
+
+struct RawBatchCtl { unsigned long long in_total; };    // Σ in_lens (zeroed before k8b_plan)
+
+struct RawBatchPlan {
+    sb_batch b;                        // the units (device descriptors)
+    uint64_t in_bytes;                 // the caller's bound on Σ in_lens (clamped to K8B_MAX_IN_BYTES)
+    uint64_t seg;                      // segment length, as for one stream
+    uint32_t* unit_blocks;             // optional: blocks decoded in parallel per unit, 0 for the one-warp path
+    RawBatchCtl* bctl;
+    RawCtl* uctl;                      // count: each unit's control record
+    uint64_t *sg_offs, *sg_tiles;      // scan over units (count + 1 entries) of their segments,
+    uint64_t *bk_offs, *bk_tiles;      // ... blocks,
+    uint64_t *wd_offs, *wd_tiles;      // ... mark words
+    uint32_t* marks;                   // per-unit slices, zeroed by each segment's k8b_chains warp
+    uint64_t *X, *Y, *ent, *ext;       // global segment list
+    uint32_t* cnt;
+    uint64_t *offs, *tiles;            // scan of cnt over nseg_cap + 1 entries
+    uint32_t nseg_cap;                 // segments the scratch holds
+    uint32_t* cut;                     // unit i: its blocks' prefix + i, nblk + 1 entries
+};
+
+// Scratch layout (host side): every array 256-byte aligned from `scratch` (null: just the size). Returns the bytes used.
+inline uint64_t k8b_carve(void* scratch, uint32_t count, uint64_t in_bytes, RawBatchPlan* q) {
+    const uint64_t in = in_bytes < K8B_MAX_IN_BYTES ? in_bytes : K8B_MAX_IN_BYTES;
+    const uint64_t units = (uint64_t)count + 1;
+    const uint64_t segs = in / K8_SEG_MIN + count;                      // Σ ceil(n_i / seg)
+    const uint64_t words = in / 32 + 2 * (uint64_t)count;               // Σ (n_i >> 5) + 2
+    const uint64_t cuts = in / 3072 + 2 * (uint64_t)count + 1;          // Σ ceil(dn_i / 65536) + 1, dn_i <= n_i * 64 / 3
+    const uintptr_t base = ((uintptr_t)scratch + 255) / 256 * 256;
+    uint64_t at = 0;
+    auto take = [&](uint64_t bytes) { const uint64_t a = at; at += (bytes + 255) / 256 * 256; return (void*)(base + a); };
+    RawBatchPlan p;
+    p.in_bytes = in;
+    p.nseg_cap = (uint32_t)segs;
+    p.bctl = (RawBatchCtl*)take(sizeof(RawBatchCtl));
+    p.uctl = (RawCtl*)take(count * sizeof(RawCtl));
+    uint64_t** scans[3][2] = {{&p.sg_offs, &p.sg_tiles}, {&p.bk_offs, &p.bk_tiles}, {&p.wd_offs, &p.wd_tiles}};
+    for (auto& sc : scans) { *sc[0] = (uint64_t*)take((units + 1) * 8); *sc[1] = (uint64_t*)take((units / K4_TILE + 3) * 8); }
+    p.marks = (uint32_t*)take(words * 4);
+    p.X = (uint64_t*)take((segs + 1) * 8);
+    p.Y = (uint64_t*)take((segs + 1) * 8);
+    p.ent = (uint64_t*)take((segs + 1) * 8);
+    p.ext = (uint64_t*)take((segs + 1) * 8);
+    p.cnt = (uint32_t*)take((segs + 1) * 4);
+    p.offs = (uint64_t*)take((segs + 2) * 8);
+    p.tiles = (uint64_t*)take(((segs + 1) / K4_TILE + 3) * 8);
+    p.cut = (uint32_t*)take(cuts * 4);
+    if (q) {
+        p.b = q->b; p.seg = q->seg; p.unit_blocks = q->unit_blocks;
+        *q = p;
+    }
+    return at + 256;
+}
+
+// exclusive prefix at i of a two-level scan
+SB_DEVICE uint64_t k8b_at(const uint64_t* offs, const uint64_t* tiles, uint64_t i) { return tiles[i / K4_TILE] + offs[i]; }
+// Σ in_lens over the bound: nothing is split
+SB_DEVICE bool k8b_over(const RawBatchPlan& q) { return q.bctl->in_total > q.in_bytes; }
+// the unit whose slice of a per-unit scan holds global index g < S(count): the last u with S(u) <= g
+SB_DEVICE uint32_t k8b_unit_of(const uint64_t* offs, const uint64_t* tiles, uint32_t count, uint64_t g) {
+    uint32_t lo = 0, hi = count;                                     // S(lo) <= g < S(hi)
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (k8b_at(offs, tiles, mid) <= g) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// unit u as one stream: its buffers, control record and slices (offs/tiles are the batch's global scan)
+SB_DEVICE RawPlan k8b_view(const RawBatchPlan& q, uint32_t u) {
+    RawPlan p;
+    p.in = unit_in(q.b, u); p.n = unit_in_len(q.b, u);
+    p.out = unit_out(q.b, u); p.cap = unit_out_cap(q.b, u);
+    p.result = nullptr;
+    p.seg = q.seg; p.nseg = (uint32_t)((p.n + q.seg - 1) / q.seg);
+    p.ctl = q.uctl + u;
+    const uint64_t s0 = k8b_at(q.sg_offs, q.sg_tiles, u);
+    p.marks = q.marks + k8b_at(q.wd_offs, q.wd_tiles, u);
+    p.X = q.X + s0; p.Y = q.Y + s0; p.ent = q.ent + s0; p.ext = q.ext + s0; p.cnt = q.cnt + s0;
+    p.offs = q.offs; p.tiles = q.tiles;
+    p.cut = q.cut + k8b_at(q.bk_offs, q.bk_tiles, u) + u;
+    return p;
+}
+
+SB_DEVICE void k8b_plan_body(const RawBatchPlan& q) {
+    const uint32_t count = q.b.count;
+    const uint64_t i = (uint64_t)block_idx() * K4_TILE + thread_idx();
+    uint32_t ns = 0, nb = 0, nw = 0;
+    uint64_t n = 0;
+    if (i < count) {
+        n = unit_in_len(q.b, (uint32_t)i);
+        const uint64_t cap = unit_out_cap(q.b, (uint32_t)i);
+        uint64_t v = 0;
+        const uint32_t hl = n ? k2_read_header(unit_in(q.b, (uint32_t)i), (uint32_t)n, &v) : 0;
+        const bool split = hl && v > kMaxBlock && v <= kMaxInput && v <= cap && v * 3 <= (n - hl) * 64;
+        RawCtl c;
+        c.decline = split ? 0u : 1u; c.dn = split ? v : 0; c.hl = hl; c.nblk = (uint32_t)((c.dn + 65535) >> 16); c.out_len = 0;
+        q.uctl[i] = c;
+        if (split) { ns = (uint32_t)((n + q.seg - 1) / q.seg); nb = c.nblk; nw = (uint32_t)((n >> 5) + 2); }
+    }
+    uint64_t t = n;
+#pragma unroll
+    for (unsigned m = 16; m; m >>= 1) t += shfl(t, lane_id() ^ m);
+    if (lane_id() == 0 && t) atomic_add(&q.bctl->in_total, (unsigned long long)t);
+    scan_local_body(count + 1, [&](uint32_t) { return ns; }, q.sg_offs, q.sg_tiles);
+    syncthreads();
+    scan_local_body(count + 1, [&](uint32_t) { return nb; }, q.bk_offs, q.bk_tiles);
+    syncthreads();
+    scan_local_body(count + 1, [&](uint32_t) { return nw; }, q.wd_offs, q.wd_tiles);
+}
+SB_DEVICE void k8b_plan_tiles_body(const RawBatchPlan& q) {
+    scan_tiles_body(q.b.count + 1, 0, q.sg_tiles);
+    syncthreads();
+    scan_tiles_body(q.b.count + 1, 0, q.bk_tiles);
+    syncthreads();
+    scan_tiles_body(q.b.count + 1, 0, q.wd_tiles);
+}
+
+// f(view, local segment k, global segment g) for every segment of the global list, one warp each
+template <class F>
+SB_DEVICE void k8b_segments(const RawBatchPlan& q, F f) {
+    if (k8b_over(q)) return;
+    const uint32_t count = q.b.count;
+    const uint64_t total = k8b_at(q.sg_offs, q.sg_tiles, count);
+    const unsigned wpb = block_dim() >> 5;
+    const uint64_t nwarps = (uint64_t)grid_dim() * wpb;
+    for (uint64_t g = (uint64_t)block_idx() * wpb + warp_id(); g < total; g += nwarps) {
+        const RawPlan p = k8b_view(q, k8b_unit_of(q.sg_offs, q.sg_tiles, count, g));
+        f(p, g - (uint64_t)(p.X - q.X), g);
+    }
+}
+
+SB_DEVICE void k8b_chains_body(const RawBatchPlan& q) {
+    k8b_segments(q, [&](const RawPlan& p, uint64_t k, uint64_t) {
+        if (k8_declined(p)) return;
+        // the segment's own words of the unit's mark slice (k8_walk marks and clears no others)
+        const uint32_t w0 = (uint32_t)(k * (p.seg >> 5));
+        const uint32_t w1 = (uint32_t)(k + 1 == p.nseg ? (p.n >> 5) + 2 : (k + 1) * (p.seg >> 5));
+        for (uint32_t w = w0 + lane_id(); w < w1; w += 32) p.marks[w] = 0;
+        syncwarp();
+        k8_chains_seg(p, k);
+    });
+}
+SB_DEVICE void k8b_merge_body(const RawBatchPlan& q) {
+    k8b_segments(q, [&](const RawPlan& p, uint64_t k, uint64_t) {
+        if (k != 0 && !k8_declined(p)) k8_merge_seg(p, k);
+    });
+}
+SB_DEVICE void k8b_stitch_body(const RawBatchPlan& q) {
+    if (k8b_over(q)) return;
+    for (uint32_t u = block_idx(); u < q.b.count; u += grid_dim()) {
+        if (q.uctl[u].decline) continue;                             // the same for every thread: only this CTA writes it
+        k8_stitch_body(k8b_view(q, u));
+        syncthreads();
+    }
+}
+SB_DEVICE void k8b_counts_body(const RawBatchPlan& q) {
+    k8b_segments(q, [&](const RawPlan& p, uint64_t k, uint64_t g) {
+        if (!k8_declined(p)) k8_counts_seg(p, k);
+        else if (lane_id() == 0) q.cnt[g] = 0;                       // scanned with the rest
+    });
+}
+SB_DEVICE void k8b_scan_local_body(const RawBatchPlan& q) {
+    const uint64_t total = k8b_over(q) ? 0 : k8b_at(q.sg_offs, q.sg_tiles, q.b.count);
+    const uint32_t* cnt = q.cnt;
+    scan_local_body(q.nseg_cap + 1, [&](uint32_t g) { return g < total ? cnt[g] : 0u; }, q.offs, q.tiles);
+}
+SB_DEVICE void k8b_scan_tiles_body(const RawBatchPlan& q) { scan_tiles_body(q.nseg_cap + 1, 0, q.tiles); }
+SB_DEVICE void k8b_cuts_body(const RawBatchPlan& q) {
+    k8b_segments(q, [&](const RawPlan& p, uint64_t k, uint64_t g) {
+        if (k8_declined(p)) return;
+        // Unit-relative positions are exact modulo 2^32 (the scan's tiles may mix units and wrap), and a split unit's
+        // output is below 2^32. A segment whose elements run past dn declines: it exists whenever the unit's true
+        // total exceeds dn, and its own base is below 2^32, so a total that wrapped cannot pass for dn.
+        const uint64_t s0 = g - k, first = k8b_at(q.offs, q.tiles, s0);
+        const uint64_t obase = (uint32_t)(k8b_at(q.offs, q.tiles, g) - first);
+        if (lane_id() == 0 && obase + p.cnt[k] > p.ctl->dn) p.ctl->decline = 1;
+        k8_cuts_seg(p, k, [&] { return (uint64_t)(uint32_t)(k8b_at(q.offs, q.tiles, s0 + p.nseg) - first); },
+                    [&] { return obase; });
+    });
+}
+SB_DEVICE void k8b_blocks_body(const RawBatchPlan& q) {
+    if (k8b_over(q)) return;
+    uint32_t* elems = (uint32_t*)smem() + warp_id() * 64;
+    const uint32_t count = q.b.count;
+    const uint64_t total = k8b_at(q.bk_offs, q.bk_tiles, count);
+    const unsigned wpb = block_dim() >> 5;
+    const uint64_t nwarps = (uint64_t)grid_dim() * wpb;
+    for (uint64_t g = (uint64_t)block_idx() * wpb + warp_id(); g < total; g += nwarps) {
+        const uint32_t u = k8b_unit_of(q.bk_offs, q.bk_tiles, count, g);
+        const RawPlan p = k8b_view(q, u);
+        if (k8_declined(p)) continue;
+        const uint64_t j = g - (uint64_t)(p.cut - q.cut - u);
+        if (p.cut[j] > p.cut[j + 1] || p.cut[j + 1] > p.n) {         // cannot happen once the cuts were accepted
+            if (lane_id() == 0) p.ctl->decline = 1;
+            continue;
+        }
+        k8_block(p, j, p.ctl->dn, elems);
+    }
+}
+SB_DEVICE void k8b_finish_body(const RawBatchPlan& q) {
+    const BatchDesc& b = q.b;
+    const bool over = k8b_over(q);
+    const unsigned wpb = block_dim() >> 5;
+    uint32_t* elems = (uint32_t*)smem() + warp_id() * 64;
+    const uint64_t nwarps = (uint64_t)grid_dim() * wpb;
+    for (uint64_t u = (uint64_t)block_idx() * wpb + warp_id(); u < b.count; u += nwarps) {
+        const uint32_t i = (uint32_t)u;
+        const RawCtl& c = q.uctl[i];
+        if (!over && !c.decline) {
+            if (lane_id() == 0) {
+                if (b.statuses) set_status(&b.statuses[i], SB_OK, 0, 0, 0);
+                if (b.out_lens) b.out_lens[i] = (uint32_t)c.dn;
+                if (q.unit_blocks) q.unit_blocks[i] = c.nblk;
+            }
+            continue;
+        }
+        if (lane_id() == 0) {
+            if (b.out_lens) b.out_lens[i] = 0;
+            if (q.unit_blocks) q.unit_blocks[i] = 0;
+        }
+        k2_decode_stream(unit_in(b, i), unit_in_len(b, i), unit_out(b, i), unit_out_cap(b, i),
+                         b.statuses ? &b.statuses[i] : nullptr, b.out_lens ? &b.out_lens[i] : nullptr, elems);
+    }
 }
 
 }  // namespace sbk

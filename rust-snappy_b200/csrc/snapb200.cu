@@ -61,6 +61,18 @@ __global__ void __launch_bounds__(1024) k8_scan_tiles_kernel(sbk::RawPlan p) { s
 __global__ void __launch_bounds__(128) k8_cuts_kernel(sbk::RawPlan p) { sbk::k8_cuts_body(p); }
 __global__ void __launch_bounds__(128) k8_blocks_kernel(sbk::RawPlan p) { sbk::k8_blocks_body(p); }
 __global__ void __launch_bounds__(32) k8_fallback_kernel(sbk::RawPlan p) { sbk::k8_fallback_body(p); }
+__global__ void __launch_bounds__(1024) k8b_plan_kernel(sbk::RawBatchPlan q) { sbk::k8b_plan_body(q); }
+__global__ void __launch_bounds__(1024) k8b_plan_tiles_kernel(sbk::RawBatchPlan q) { sbk::k8b_plan_tiles_body(q); }
+// the cap lets ptxas keep the unit lookup and the segment's mark range in registers (at 32 it spilled)
+__global__ void __launch_bounds__(128, 12) k8b_chains_kernel(sbk::RawBatchPlan q) { sbk::k8b_chains_body(q); }
+__global__ void __launch_bounds__(128) k8b_merge_kernel(sbk::RawBatchPlan q) { sbk::k8b_merge_body(q); }
+__global__ void __launch_bounds__(sbk::K8_STITCH_THREADS) k8b_stitch_kernel(sbk::RawBatchPlan q) { sbk::k8b_stitch_body(q); }
+__global__ void __launch_bounds__(128) k8b_counts_kernel(sbk::RawBatchPlan q) { sbk::k8b_counts_body(q); }
+__global__ void __launch_bounds__(1024) k8b_scan_local_kernel(sbk::RawBatchPlan q) { sbk::k8b_scan_local_body(q); }
+__global__ void __launch_bounds__(1024) k8b_scan_tiles_kernel(sbk::RawBatchPlan q) { sbk::k8b_scan_tiles_body(q); }
+__global__ void __launch_bounds__(128) k8b_cuts_kernel(sbk::RawBatchPlan q) { sbk::k8b_cuts_body(q); }
+__global__ void __launch_bounds__(128) k8b_blocks_kernel(sbk::RawBatchPlan q) { sbk::k8b_blocks_body(q); }
+__global__ void __launch_bounds__(128) k8b_finish_kernel(sbk::RawBatchPlan q) { sbk::k8b_finish_body(q); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -484,6 +496,45 @@ int launch_raw_decode(Ctx& c, const sbk::RawPlan& p, cudaStream_t st, sb_error* 
     return 0;
 }
 
+
+// ---- raw batch decode (K8 over every unit with more than one block, one warp for the rest)
+uint64_t raw_batch_ws_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k8b_carve(nullptr, count, in_bytes, nullptr); }
+int launch_raw_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_unit_blocks, void* scratch, cudaStream_t st,
+                     sb_error* err) {
+    if (b.count == 0) return 0;
+    sbk::RawBatchPlan q;
+    memset(&q, 0, sizeof q);
+    q.b = b; q.seg = sbk::k8_seg_len(k8_want_seg()); q.unit_blocks = d_unit_blocks;
+    sbk::k8b_carve(scratch, b.count, in_bytes, &q);
+    // grids: warps over the segment / block / unit lists, whose true lengths are on the device
+    auto warps = [&](uint64_t n, unsigned per_sm) {
+        const uint64_t g = (n + 3) / 4, most = (uint64_t)per_sm * c.sms;
+        return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most;
+    };
+    const uint64_t in = q.in_bytes;
+    CK(cudaMemsetAsync(q.bctl, 0, sizeof(sbk::RawBatchCtl), st));
+    const unsigned utiles = (unsigned)(((uint64_t)b.count + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    k8b_plan_kernel<<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k8b_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    const unsigned segw = warps(q.nseg_cap, 16);
+    k8b_chains_kernel<<<segw, 128, 0, st>>>(q);
+    k8b_merge_kernel<<<segw, 128, 0, st>>>(q);
+    const unsigned sgrid = b.count < (uint32_t)(8 * c.sms) ? b.count : (unsigned)(8 * c.sms);
+    k8b_stitch_kernel<<<sgrid, sbk::K8_STITCH_THREADS, sbk::K8_STITCH_THREADS * 16 + 16, st>>>(q);
+    k8b_counts_kernel<<<segw, 128, 0, st>>>(q);
+    const unsigned ctiles = (unsigned)(((uint64_t)q.nseg_cap + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    k8b_scan_local_kernel<<<ctiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k8b_scan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    k8b_cuts_kernel<<<segw, 128, 0, st>>>(q);
+    k8b_blocks_kernel<<<warps(in / 3072 + b.count, 16), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    // the one-warp pass, sized like launch_k2
+    static const int per_sm = getenv("SNAPB200_K2_CTAS") ? atoi(getenv("SNAPB200_K2_CTAS")) : K2_DEFAULT_CTAS_PER_SM;
+    k8b_finish_kernel<<<warps(b.count, per_sm), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    g_launches += 11;
+    CK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 // =========================================================================
@@ -557,7 +608,13 @@ int sb_reserve(size_t wave_units, size_t wave_in_bytes, size_t wave_out_bytes, s
             CK(l.status[b].need(wave_units * sizeof(sb_error) + 64));
             CK(l.ptrs_in[b].need(wave_units * 8 + 8));
             CK(l.ptrs_out[b].need(wave_units * 8 + 8));
-            CK(l.ws[b].need(align_up((wave_units / sbk::K4_TILE + 3) * 8, 256) + align_up((wave_units + 1) * 8, 256) + 1024));
+            size_t ws = align_up((wave_units / sbk::K4_TILE + 3) * 8, 256) + align_up((wave_units + 1) * 8, 256) + 1024;
+            // decode waves holding units of more than one block run K8 over the batch in this scratch
+            if (ln == LANE_DEC && wave_units) {
+                const size_t rb = raw_batch_ws_bytes((uint32_t)wave_units, wave_out_bytes + wave_units * 16);
+                if (rb > ws) ws = rb;
+            }
+            CK(l.ws[b].need(ws));
             rc = need_pinned(l, b, wave_units * 24 + 64, err); if (rc) return rc;
             rc = need_pinned(l, 2 + b, wave_units * (4 + sizeof(sb_error)) + 64, err); if (rc) return rc;
         }
@@ -579,6 +636,24 @@ int sb_decompress_device_ws(const uint8_t* d_in, uint64_t n, uint8_t* d_out, uin
     int rc = get_ctx(&c, err);
     if (rc) return rc;
     rc = launch_raw_decode(*c, make_raw_plan(d_in, n, d_out, cap, d_result, scratch, k8_want_seg()), (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_decompress_batch_scratch_bytes(uint32_t count, uint64_t in_bytes) { return raw_batch_ws_bytes(count, in_bytes); }
+
+int sb_decompress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t* d_unit_blocks, void* scratch,
+                                  uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if (!batch || !batch->out_lens || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K8B_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K8B_MAX_COUNT);
+    if (batch->count == 0) { ok(err); return 0; }
+    const uint64_t need = raw_batch_ws_bytes(batch->count, in_bytes);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_raw_batch(*c, *batch, in_bytes, d_unit_blocks, scratch, (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;
@@ -993,7 +1068,20 @@ int sb_decompress_batch_host(const uint8_t* in_base, const uint64_t* in_offs, co
         bt.in_ptrs = (const uint8_t* const*)l.ptrs_in[b].p; bt.in_lens = l.caps[b].as<uint32_t>();
         bt.out_ptrs = (uint8_t* const*)l.ptrs_out[b].p; bt.out_caps = l.caps[b].as<uint32_t>() + w.count;
         bt.out_lens = l.lens[b].as<uint32_t>(); bt.statuses = l.status[b].as<sb_error>(); bt.count = (uint32_t)w.count;
-        rc = launch_k2(*c, bt, l.s_compute, err);
+        // a unit whose header announces more than one block (only possible where its cap allows it) is split by K8
+        bool multi = false;
+        for (size_t k = 0; k < w.count && !multi; k++) {
+            const size_t i = w.first + k;
+            uint64_t v = 0;
+            multi = out_caps[i] > SB_MAX_BLOCK && get_varint(in_base + in_offs[i], in_lens[i], &v) && v > SB_MAX_BLOCK;
+        }
+        if (multi) {
+            const uint64_t wsb = raw_batch_ws_bytes(bt.count, w.in_bytes);
+            CK(l.ws[b].need(wsb));
+            rc = launch_raw_batch(*c, bt, w.in_bytes, nullptr, l.ws[b].p, l.s_compute, err);
+        } else {
+            rc = launch_k2(*c, bt, l.s_compute, err);
+        }
         if (rc) return rc;
         { int prc = need_pinned(l, 2 + b, w.count * (4 + sizeof(sb_error)) + 64, err); if (prc) return prc; }
         sb_error* pst = (sb_error*)l.pinned[2 + b];
