@@ -156,6 +156,26 @@ int sb_decompress_batch_device(const sb_batch* batch, void* stream, sb_error* er
 uint64_t sb_decompress_batch_scratch_bytes(uint32_t count, uint64_t in_bytes);
 int sb_decompress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t* d_unit_blocks,
                                   void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
+/* Raw compress of units of ANY length: unit i becomes exactly what Encoder::compress(input_i, &mut output_i[..cap_i])
+ * produces (src/compress.rs:99-154), cap_i = out_caps[i] or the uniform cap; the same addressing as the other batch
+ * calls, and a uniform length over 65536 is legal. Every unit is cut into its 64 KB blocks and the blocks of all units
+ * are compressed in one launch, then each unit's varint header and block bodies are assembled in its output. Per unit:
+ *   Ok: out_lens[i] = the stream's length (an empty unit is the one byte 0x00).
+ *   TooBig{given=n, max=2^32-1} when max_compress_len(n) == 0 (n > 3,681,400,511);
+ *   BufferTooSmall{given=cap_i, min=max_compress_len(n)} when cap_i is smaller.
+ *   A unit that is not compressed has out_lens[i] = 0 (every stream is at least one byte), and neither its input nor its
+ *   output is touched. statuses may be NULL.
+ *   in_bytes: the caller's bound on the sum of in_lens over units of MORE than 65536 bytes (0 for a batch of <= 64 KB
+ *     units); the scratch, sb_compress_batch_scratch_bytes(count, in_bytes) bytes, depends on nothing else. When those
+ *     lengths sum to more than in_bytes on the device, every such unit gets SB_E_INVALID{a=sum, b=in_bytes} and
+ *     out_lens 0; units of at most 65536 bytes are still compressed. Rejected units do not count towards the sum.
+ * Stream ordered, no allocation, no host synchronisation; with count 1 it is the device-resident sb_compress. Null
+ * pointers (batch, out_lens, scratch), count >= 2^31, a bound whose block count does not fit one launch
+ * (sb_compress_batch_scratch_bytes returns UINT64_MAX) and scratch that is too small are SB_E_INVALID with nothing
+ * launched; count == 0 does nothing. Like sb_compress_batch_device, launches on different streams are ordered. */
+uint64_t sb_compress_batch_scratch_bytes(uint32_t count, uint64_t in_bytes);
+int sb_compress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, void* scratch, uint64_t scratch_bytes,
+                                void* stream, sb_error* err);
 /* Masked CRC-32C of each unit (frame chunks): out_lens[i] receives the CRC. */
 int sb_crc32c_masked_batch_device(const sb_batch* batch, void* stream, sb_error* err);
 

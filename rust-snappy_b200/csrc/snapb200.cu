@@ -21,6 +21,7 @@
 #include "k5_frame_decode.cuh"
 #include "k7_frame_index.cuh"
 #include "k8_raw_split.cuh"
+#include "k9_raw_batch_compress.cuh"
 
 namespace {
 
@@ -73,6 +74,14 @@ __global__ void __launch_bounds__(1024) k8b_scan_tiles_kernel(sbk::RawBatchPlan 
 __global__ void __launch_bounds__(128) k8b_cuts_kernel(sbk::RawBatchPlan q) { sbk::k8b_cuts_body(q); }
 __global__ void __launch_bounds__(128) k8b_blocks_kernel(sbk::RawBatchPlan q) { sbk::k8b_blocks_body(q); }
 __global__ void __launch_bounds__(128) k8b_finish_kernel(sbk::RawBatchPlan q) { sbk::k8b_finish_body(q); }
+__global__ void __launch_bounds__(256) k9_plan_kernel(sbk::RawCompressPlan q) { sbk::k9_plan_body(q); }
+__global__ void __launch_bounds__(1024) k9_scan_local_kernel(sbk::RawCompressPlan q) { sbk::k9_scan_local_body(q); }
+__global__ void __launch_bounds__(1024) k9_scan_tiles_kernel(sbk::RawCompressPlan q) { sbk::k9_scan_tiles_body(q); }
+__global__ void __launch_bounds__(256) k9_fill_kernel(sbk::RawCompressPlan q) { sbk::k9_fill_body(q); }
+__global__ void __launch_bounds__(1024) k9_bscan_local_kernel(sbk::RawCompressPlan q) { sbk::k9_bscan_local_body(q); }
+__global__ void __launch_bounds__(1024) k9_bscan_tiles_kernel(sbk::RawCompressPlan q) { sbk::k9_bscan_tiles_body(q); }
+__global__ void __launch_bounds__(256) k9_gather_kernel(sbk::RawCompressPlan q) { sbk::k9_gather_body(q); }
+__global__ void __launch_bounds__(256) k9_finish_kernel(sbk::RawCompressPlan q) { sbk::k9_finish_body(q); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -535,6 +544,35 @@ int launch_raw_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_u
     return 0;
 }
 
+
+// ---- raw batch compress (units of any length: every block of the batch in one K1 launch, assembled per unit)
+uint64_t raw_compress_ws_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k9_carve(nullptr, count, in_bytes, nullptr); }
+int launch_raw_compress(Ctx& c, const sb_batch& b, uint64_t in_bytes, void* scratch, cudaStream_t st, sb_error* err) {
+    sbk::RawCompressPlan q;
+    memset(&q, 0, sizeof q);
+    q.b = b;
+    sbk::k9_carve(scratch, b.count, in_bytes, &q);
+    auto threads = [](uint64_t n, unsigned per) { return (unsigned)((n + per - 1) / per); };
+    CK(cudaMemsetAsync(q.ctl, 0, sizeof(sbk::RawCompressCtl), st));
+    k9_plan_kernel<<<threads(b.count, 256), 256, 0, st>>>(q);
+    k9_scan_local_kernel<<<threads((uint64_t)b.count + 1, sbk::K4_TILE), sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k9_scan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    k9_fill_kernel<<<threads(q.nk, 256), 256, 0, st>>>(q);
+    g_launches += 4;
+    CK(cudaGetLastError());
+    int rc = launch_k1(c, sbk::k9_k1_batch(q), 0u, nullptr, st, err);
+    if (rc) return rc;
+    k9_bscan_local_kernel<<<threads((uint64_t)q.nslot + 1, sbk::K4_TILE), sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k9_bscan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    // warps over the slot list, whose true length is on the device
+    const uint64_t gw = ((uint64_t)q.nslot + 7) / 8, most = (uint64_t)16 * c.sms;
+    k9_gather_kernel<<<gw == 0 ? 1u : gw < most ? (unsigned)gw : (unsigned)most, 256, 0, st>>>(q);
+    k9_finish_kernel<<<threads(b.count, 256), 256, 0, st>>>(q);
+    g_launches += 4;
+    CK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 // =========================================================================
@@ -654,6 +692,25 @@ int sb_decompress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint
     int rc = get_ctx(&c, err);
     if (rc) return rc;
     rc = launch_raw_batch(*c, *batch, in_bytes, d_unit_blocks, scratch, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_compress_batch_scratch_bytes(uint32_t count, uint64_t in_bytes) { return raw_compress_ws_bytes(count, in_bytes); }
+
+int sb_compress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, void* scratch, uint64_t scratch_bytes, void* stream,
+                                sb_error* err) {
+    if (!batch || !batch->out_lens || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K9_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K9_MAX_COUNT);
+    if (batch->count == 0) { ok(err); return 0; }
+    const uint64_t need = raw_compress_ws_bytes(batch->count, in_bytes);
+    if (need == ~0ull) return fail(err, SB_E_INVALID, batch->count, in_bytes);   // more blocks than one K1 launch takes
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_raw_compress(*c, *batch, in_bytes, scratch, (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;
