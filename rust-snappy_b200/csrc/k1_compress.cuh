@@ -40,12 +40,14 @@
 #if defined(K1_PROFILE) && defined(__CUDACC__)
 // Optional phase timers for kernel archaeology (tools/k1_phase_profile.sh builds a separate
 // library with -DK1_PROFILE; the product build has none of this).
-__device__ unsigned long long g_k1_prof[16];
+// [0..11]: cycles per phase (K1_TICK slots), [12 + s]: parser warps per scheduler, [16 + k]: K1_COUNT(k) windows
+__device__ unsigned long long g_k1_prof[18];
 #define K1_TICK(slot) do { const long long _now = clock64(); if (sbk::lane_id() == 0) k1_acc[slot] += (unsigned long long)(_now - k1_t0); k1_t0 = _now; } while (0)
-#define K1_PROF_DECL unsigned long long k1_acc[12] = {0,0,0,0,0,0,0,0,0,0,0,0}; long long k1_t0 = clock64();
+#define K1_COUNT(k) do { if (sbk::lane_id() == 0) k1_acc[12 + (k)]++; } while (0)
+#define K1_PROF_DECL unsigned long long k1_acc[14] = {0,0,0,0,0,0,0,0,0,0,0,0,0,0}; long long k1_t0 = clock64();
 #define K1_PROF_ARGS , unsigned long long* k1_acc, long long& k1_t0
 #define K1_PROF_PASS , k1_acc, k1_t0
-#define K1_PROF_FLUSH do { if (sbk::lane_id() == 0) for (int _i = 0; _i < 12; _i++) atomicAdd(&g_k1_prof[_i], k1_acc[_i]); } while (0)
+#define K1_PROF_FLUSH do { if (sbk::lane_id() == 0) for (int _i = 0; _i < 14; _i++) atomicAdd(&g_k1_prof[_i < 12 ? _i : _i + 4], k1_acc[_i]); } while (0)
 // [12 + s]: parser warps the hardware placed on scheduler s (%warpid & 3), one count per warp and launch
 #define K1_PROF_CENSUS(is_parser) do { unsigned _hw; asm volatile("mov.u32 %0, %%warpid;" : "=r"(_hw)); \
     if ((is_parser) && sbk::lane_id() == 0) atomicAdd(&g_k1_prof[12 + (_hw & 3u)], 1ull); } while (0)
@@ -56,7 +58,16 @@ __device__ unsigned long long g_k1_prof[16];
 #define K1_PROF_ARGS
 #define K1_PROF_PASS
 #define K1_PROF_FLUSH do { } while (0)
+#if defined(SB_EMU)
+// CPU warp-emulator build (tests/emu): the same window counts, readable by the tests through the symbol
+extern "C" { __attribute__((weak)) unsigned long long sb_emu_k1_windows[3]; }
+#define K1_COUNT(k) do { if (sbk::lane_id() == 0) sb_emu_k1_windows[k]++; } while (0)
+#else
+#define K1_COUNT(k) do { } while (0)
 #endif
+#endif
+// K1_COUNT: [0] fast-path windows whose probe the previous window issued (hoisted), [1] probes issued at the loop top;
+// emulator build only: [2] probes whose table slot changed between the read and the use (must stay 0)
 
 namespace sbk {
 
@@ -149,6 +160,11 @@ struct K1State {
     uint32_t skip;     // scan state (src/compress.rs:204-211); meaningful when !rematch
     bool rematch;      // true: a copy just ended at s and s-1 is already inserted (:285-301 first half)
 };
+// the window at w (holding st.s) runs on the parser's fast path: well inside the block, and a scan still probes
+// every position
+SB_DEVICE bool k1_fast(uint32_t w, const K1State& st, uint32_t s_limit) {
+    return w + 36 < s_limit && (st.rematch || st.skip < 64);
+}
 
 #define K1_HASH(x) (((uint32_t)(x) * 0x1E35A7BDu) >> shift)
 // after a copy ends at e: `if s >= s_limit return` else insert e-1 (:275-295)
@@ -271,21 +287,28 @@ SB_DEVICE uint32_t k1_double(uint32_t E, bool eq, uint32_t L) {
     return M;
 }
 
-SB_DEVICE K1Pre k1_eval(const uint8_t* win, const uint16_t* table, unsigned shift, uint32_t w, const K1Seq* seq K1_PROF_ARGS) {
-    const uint32_t p = w + lane_id();
-    K1Pre r;
-    const uintptr_t aa = (uintptr_t)(win + p);
-    const unsigned ash = (unsigned)(aa & 3u) * 8;
-    uint32_t a0, a1, a2, a3, a4;
-    if (seq && seq->w == w) { a0 = seq->a0; a1 = seq->a1; a2 = seq->a2; a3 = seq->a3; a4 = seq->a4; }
-    else { const K1Seq q = k1_fetch_seq(win, w); a0 = q.a0; a1 = q.a1; a2 = q.a2; a3 = q.a3; a4 = q.a4; }
-    const uint32_t cur = funnel_r(a0, a1, ash);
-    r.h = K1_HASH(cur);
+// A window's probe between its issue and its use: the lane's hash, the table slot and the
+// candidate's five aligned words, whose loads may still be in flight.
+struct K1Probe { uint32_t h, c, b0, b1, b2, b3, b4; };
+SB_DEVICE K1Probe k1_probe_issue(const uint8_t* win, const uint16_t* table, unsigned shift, const K1Seq& q) {
+    const unsigned ash = (unsigned)((uintptr_t)(win + q.w + lane_id()) & 3u) * 8;
+    K1Probe r;
+    r.h = K1_HASH(funnel_r(q.a0, q.a1, ash));
     r.c = table[r.h];
-    const uintptr_t ba = (uintptr_t)(win + r.c);
-    const uint32_t* bw = (const uint32_t*)(ba & ~(uintptr_t)3);
-    const unsigned bsh = (unsigned)(ba & 3u) * 8;
-    const uint32_t b0 = bw[0], b1 = bw[1], b2 = bw[2], b3 = bw[3], b4 = bw[4];
+    const uint32_t* bw = (const uint32_t*)((uintptr_t)(win + r.c) & ~(uintptr_t)3);
+    r.b0 = bw[0]; r.b1 = bw[1]; r.b2 = bw[2]; r.b3 = bw[3]; r.b4 = bw[4];
+    return r;
+}
+// compare, match length, hit ballots and pointer doubling of a probe issued on the words `q`
+SB_DEVICE K1Pre k1_probe_complete(const uint8_t* win, const K1Seq& q, const K1Probe& pb) {
+    const unsigned ash = (unsigned)((uintptr_t)(win + q.w + lane_id()) & 3u) * 8;
+    const uint32_t a0 = q.a0, a1 = q.a1, a2 = q.a2, a3 = q.a3, a4 = q.a4;
+    const uint32_t b0 = pb.b0, b1 = pb.b1, b2 = pb.b2, b3 = pb.b3, b4 = pb.b4;
+    const unsigned bsh = (unsigned)((uintptr_t)(win + pb.c) & 3u) * 8;
+    const uint32_t cur = funnel_r(a0, a1, ash);
+    K1Pre r;
+    r.h = pb.h;
+    r.c = pb.c;
     r.eq = cur == funnel_r(b0, b1, bsh);
     // match length, branch-free: bytes 4..15 of both sides, first differing byte wins
     {
@@ -299,21 +322,22 @@ SB_DEVICE K1Pre k1_eval(const uint8_t* win, const uint16_t* table, unsigned shif
     }
     r.E = ballot(r.eq);
     r.longs = ballot(r.eq && r.L == 16);
-    K1_TICK(1);                                                  // [1] probe: hash, table, candidate words, compare
     r.M = k1_double(r.E, r.eq, r.L);
-    K1_TICK(2);                                                  // [2] pointer doubling
     return r;
 }
 
 // Finish one window from a probe result that is known to be current for every lane
 // from the entry position on. Returns false (state untouched, table restored) when
-// the window must be replayed serially.
+// the window must be replayed serially. `nxt` holds the sequential words prefetched for w + 32;
+// `hoisted` tells whether the next window's probe was issued into `nextp` (DESIGN.md section 4).
 // GT: the table lives in global memory (L2) instead of shared memory -- a re-read costs a
 // full L2 round trip there, so slot clashes are found by comparing hashes across lanes.
 template <bool GT>
 SB_DEVICE bool k1_finish(const uint8_t* win, uint32_t n, uint16_t* table, unsigned shift, uint32_t s_limit,
-                         K1State& st, const K1Ring& ring, K1Prod& head, const K1Pre& pre, const K1Seq* nxt K1_PROF_ARGS) {
+                         K1State& st, const K1Ring& ring, K1Prod& head, const K1Pre& pre, const K1Seq* nxt,
+                         K1Probe& nextp, bool& hoisted K1_PROF_ARGS) {
     const unsigned lane = lane_id();
+    hoisted = false;
     const uint32_t w = st.s & ~31u, i0 = st.s - w, p = w + lane;
     const uint32_t h = pre.h, c = pre.c, E = pre.E;
     const bool eq = pre.eq;
@@ -400,41 +424,48 @@ SB_DEVICE bool k1_finish(const uint8_t* win, uint32_t n, uint16_t* table, unsign
         }
     }
     K1_TICK(5);                                                  // [5] commit + verify (+ clash handling)
-    // ---- publish the copies and leave the window
+    // ---- exit state and copy-end insert
     const uint32_t ncopy = popc(CS);
-    if (ncopy) {
-        k1_wait_space(ring, head, ncopy);
-        if (taken) ring.ev[(head.head + popc(CS & ((1u << lane) - 1u))) & (ring.size - 1)] = k1_event(p, L, p - c);
-        head.head += ncopy;
-        if (head.head - head.published >= K1_PUBLISH) k1_publish(ring, head);
-        K1_TICK(6);                                              // [6] event ring
-        const unsigned last = 31 - clz(CS);
-        const uint32_t e_last = last + shfl(L, last);
-        if (e_last >= 32) {
-            st.s = w + e_last; st.rematch = true;
-            if (e_last >= 33) {                                   // e-1 lies beyond this window
-                if (nxt && nxt->w == w + 32 && e_last <= 64) {
-                    // ... but inside the next one, whose sequential words are already prefetched: take
-                    // its hash from the lane that holds it instead of paying a global load (:293-295)
-                    if (st.s < s_limit) {
-                        const unsigned nsh = (unsigned)((uintptr_t)(win + nxt->w + lane) & 3u) * 8;
-                        const uint32_t hsel = shfl(K1_HASH(funnel_r(nxt->a0, nxt->a1, nsh)), e_last - 33);
-                        syncwarp();
-                        if (lane == 0) table[hsel] = (uint16_t)(st.s - 1);
-                        syncwarp();
-                    }
-                } else {
-                    k1_preinsert(win, table, shift, s_limit, st.s);
+    const unsigned last = ncopy ? 31 - clz(CS) : 0;
+    const uint32_t e_last = ncopy ? last + shfl(L, last) : 0;
+    if (ncopy && e_last >= 32) {
+        st.s = w + e_last; st.rematch = true;
+        if (e_last >= 33) {                                       // e-1 lies beyond this window
+            if (nxt->w == w + 32 && e_last <= 64) {
+                // ... but inside the next one, whose sequential words are already prefetched: take
+                // its hash from the lane that holds it instead of paying a global load (:293-295)
+                if (st.s < s_limit) {
+                    const unsigned nsh = (unsigned)((uintptr_t)(win + nxt->w + lane) & 3u) * 8;
+                    const uint32_t hsel = shfl(K1_HASH(funnel_r(nxt->a0, nxt->a1, nsh)), e_last - 33);
+                    syncwarp();
+                    if (lane == 0) table[hsel] = (uint16_t)(st.s - 1);
+                    syncwarp();
                 }
+            } else {
+                k1_preinsert(win, table, shift, s_limit, st.s);
             }
-        } else {
-            st.s = w + 32; st.rematch = false; st.skip = 32 + (31 - e_last);
         }
+    } else if (ncopy) {
+        st.s = w + 32; st.rematch = false; st.skip = 32 + (31 - e_last);
     } else {
         st.skip = st.rematch ? 32 + (31 - i0) : st.skip + (32 - i0);
         st.s = w + 32; st.rematch = false;
     }
+    const uint32_t slot = popc(CS & ((1u << lane) - 1u));     // this lane's event among the window's copies
     K1_TICK(7);                                                  // [7] exit state / copy-end insert
+    // ---- the next window's probe. Every table store of this window is done, so when the next window is w + 32
+    // on the fast path its probe reads exactly the table it would read later: issue it now so that its candidate
+    // loads overlap the ring stores and the next window's prefetch (k1_parse keeps such windows in its inner loop)
+    hoisted = nxt->w == w + 32 && (st.s & ~31u) == w + 32 && k1_fast(w + 32, st, s_limit);
+    if (hoisted) nextp = k1_probe_issue(win, table, shift, *nxt);
+    // ---- publish the copies
+    if (ncopy) {
+        k1_wait_space(ring, head, ncopy);
+        if (taken) ring.ev[(head.head + slot) & (ring.size - 1)] = k1_event(p, L, p - c);
+        head.head += ncopy;
+        if (head.head - head.published >= K1_PUBLISH) k1_publish(ring, head);
+    }
+    K1_TICK(6);                                                  // [6] probe issue + event ring
     return true;
 }
 
@@ -456,10 +487,10 @@ SB_DEVICE void k1_parse(const uint8_t* win, uint32_t n, uint16_t* table, const K
     K1State st;
     st.s = 1; st.skip = 32; st.rematch = false;
     for (;;) {
-        const uint32_t w = st.s & ~31u;
+        uint32_t w = st.s & ~31u;
         bool finished;
         // fast-path test first: when it holds (w + 36 < s_limit, stride 1) neither end-of-block test can
-        const bool fast = w + 36 < s_limit && (st.rematch || st.skip < 64);
+        const bool fast = k1_fast(w, st, s_limit);
         if (!fast && (st.rematch ? st.s >= s_limit : st.s + (st.skip >> 5) > s_limit)) finished = true;
         else {
             bool ok = false;
@@ -467,9 +498,37 @@ SB_DEVICE void k1_parse(const uint8_t* win, uint32_t n, uint16_t* table, const K
                 K1Seq nxt = seq;
                 if (w + 100 < n) nxt = k1_fetch_seq(win, w + 32);   // issue next window's loads now
                 K1_TICK(0);                                          // [0] loop top / state checks / prefetch issue
-                const K1Pre pre = k1_eval(win, table, shift, w, &seq K1_PROF_PASS);
-                seq = nxt;
-                ok = k1_finish<GT>(win, n, table, shift, s_limit, st, ring, prod, pre, &seq K1_PROF_PASS);
+                K1Seq cur = seq.w == w ? seq : k1_fetch_seq(win, w);
+                K1Probe pb = k1_probe_issue(win, table, shift, cur);
+                K1_COUNT(1);
+                // While a window issues its successor's probe (`hoisted`), the successor runs in this inner loop
+                // and not from the loop top: there the compiler joins all paths of the parse and waits for every
+                // load in flight, which would put the candidate loads back on the critical path. For the same
+                // reason the successor's own prefetch is issued only after its candidates are compared.
+                K1_TICK(11);                                         // [11] probe issue (loop top)
+#ifdef SB_EMU
+                if (table[pb.h] != (uint16_t)pb.c) K1_COUNT(2);
+#endif
+                K1Pre pre = k1_probe_complete(win, cur, pb);
+                K1_TICK(1);                                          // [1] candidate wait, compare, doubling
+                for (;;) {
+                    seq = nxt;
+                    bool hoisted;
+                    ok = k1_finish<GT>(win, n, table, shift, s_limit, st, ring, prod, pre, &seq, pb, hoisted K1_PROF_PASS);
+                    if (!hoisted) break;
+                    w += 32;                                         // == st.s & ~31u, on the fast path
+                    cur = seq;
+                    K1_TICK(0);
+                    K1_COUNT(0);
+#ifdef SB_EMU
+                    if (table[pb.h] != (uint16_t)pb.c) K1_COUNT(2);
+#endif
+                    pre = k1_probe_complete(win, cur, pb);
+                    K1_TICK(1);
+                    // unconditional (the current window when w + 32 is too close to the end): a conditional load
+                    // would become register moves that wait for it
+                    nxt = k1_fetch_seq(win, w + 100 < n ? w + 32 : w);
+                }
             }
             if (!ok) { K1_TICK(8); finished = k1_serial(win, n, table, shift, s_limit, st, w + 32, ring, prod); K1_TICK(9); }   // [9] serial path
             else finished = false;

@@ -1416,10 +1416,10 @@ int snappy_uncompressed_length(const char* compressed, size_t compressed_length,
 
 #ifdef K1_PROFILE
 // profile build only (tools/k1_phase_profile.sh): read / reset the parser phase timers
-int sb_debug_k1_profile(unsigned long long* out16, int reset) {
+int sb_debug_k1_profile(unsigned long long* out18, int reset) {
     cudaDeviceSynchronize();
-    if (out16 && cudaMemcpyFromSymbol(out16, g_k1_prof, sizeof(unsigned long long) * 16) != cudaSuccess) return 1;
-    if (reset) { unsigned long long z[16] = {0}; if (cudaMemcpyToSymbol(g_k1_prof, z, sizeof z) != cudaSuccess) return 1; }
+    if (out18 && cudaMemcpyFromSymbol(out18, g_k1_prof, sizeof(unsigned long long) * 18) != cudaSuccess) return 1;
+    if (reset) { unsigned long long z[18] = {0}; if (cudaMemcpyToSymbol(g_k1_prof, z, sizeof z) != cudaSuccess) return 1; }
     return 0;
 }
 #endif

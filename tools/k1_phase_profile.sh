@@ -30,18 +30,22 @@ L.sb_generate_blocks_device(t_text.data_ptr(), len(text), t_in.data_ptr(), BLOCK
 b = snap._lib.SbBatch(); b.in_base, b.in_stride, b.in_len_uniform = t_in.data_ptr(), BLOCK, BLOCK
 b.out_base, b.out_stride, b.out_cap_uniform, b.out_lens, b.count = t_c.data_ptr(), STRIDE, STRIDE, cl.data_ptr(), n
 L.sb_compress_batch_device(C.byref(b), st, C.byref(err)); torch.cuda.synchronize()
-out = (C.c_ulonglong * 16)()
+out = (C.c_ulonglong * 18)()
 L.sb_debug_k1_profile(out, 1)
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 e0.record(); L.sb_compress_batch_device(C.byref(b), st, C.byref(err)); e1.record(); torch.cuda.synchronize()
 L.sb_debug_k1_profile(out, 0)
-names = ["loop top/prefetch", "probe (hash,table,cand,compare)", "pointer doubling", "entry->taken copies", "interiors/inserted mask",
-         "commit+verify(+clash)", "event ring", "exit state/copy-end insert", "(pre-serial)", "serial path", "block end"]
-tot = sum(out[i] for i in range(11))
+names = ["loop top/prefetch", "probe: candidate wait, compare", "pointer doubling", "entry->taken copies", "interiors/inserted mask",
+         "commit+verify(+clash)", "probe issue + event ring", "exit state/copy-end insert", "(pre-serial)", "serial path",
+         "block end", "probe issue at the loop top"]
+tot = sum(out[i] for i in range(12))
 windows = n * (BLOCK // 32)
 print("lib %s: kernel %.2f ms, %.2f GB/s; parser cycles per 32-byte window: %.0f"
       % (os.path.basename(os.environ["SNAPB200_LIB"]), e0.elapsed_time(e1), n * BLOCK / e0.elapsed_time(e1) / 1e6, tot / windows))
-for i in range(11):
+for i in range(12):
     print("  [%2d] %-34s %6.1f%%  %7.0f cyc/window" % (i, names[i], 100.0 * out[i] / tot, out[i] / windows))
 print("parser warps per scheduler (%%warpid & 3 = 0..3): %s" % [out[12 + s] for s in range(4)])
+fw = out[16] + out[17]
+print("fast-path windows: %d; probe issued by the previous window (hoisted): %d (%.1f%%), at the loop top: %d"
+      % (fw, out[16], 100.0 * out[16] / max(fw, 1), out[17]))
 PY
