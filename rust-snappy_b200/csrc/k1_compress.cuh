@@ -96,8 +96,9 @@ struct K1Ring {
     uint32_t* ctrl;      // [0]=head (produced), [1]=tail (consumed), [6..7]=producer counters between units, [8]=unit
     uint32_t size;
 };
+// pos | len << 17 | off << 34, built as its two 32-bit halves (pos, len <= 65536: len << 17 carries into the high word)
 SB_DEVICE uint64_t k1_event(uint32_t pos, uint32_t len, uint32_t off) {
-    return (uint64_t)pos | ((uint64_t)len << 17) | ((uint64_t)off << 34);
+    return (uint64_t)(pos | (len << 17)) | ((uint64_t)((len >> 15) | (off << 2)) << 32);
 }
 // producer side. The parser keeps private copies of the ring counters and only
 // touches the shared ones when it has to: `tail_seen` is refreshed when the ring
@@ -315,10 +316,10 @@ SB_DEVICE K1Pre k1_probe_complete(const uint8_t* win, const K1Seq& q, const K1Pr
         const uint32_t x4 = funnel_r(a1, a2, ash) ^ funnel_r(b1, b2, bsh);
         const uint32_t x8 = funnel_r(a2, a3, ash) ^ funnel_r(b2, b3, bsh);
         const uint32_t x12 = funnel_r(a3, a4, ash) ^ funnel_r(b3, b4, bsh);
-        const uint32_t l4 = 4 + ((uint32_t)(ffs(x4) - 1) >> 3);       // valid when x4 != 0
-        const uint32_t l8 = 8 + ((uint32_t)(ffs(x8) - 1) >> 3);
-        const uint32_t l12 = x12 ? 12 + ((uint32_t)(ffs(x12) - 1) >> 3) : 16;
-        r.L = x4 ? l4 : x8 ? l8 : l12;
+        // the first word that differs and its base are selected first: one find-first-set instead of three
+        const uint32_t x = x4 ? x4 : x8 ? x8 : x12;
+        const uint32_t lb = x4 ? 4u : x8 ? 8u : 12u;
+        r.L = x ? lb + ((uint32_t)(ffs(x) - 1) >> 3) : 16;
     }
     r.E = ballot(r.eq);
     r.longs = ballot(r.eq && r.L == 16);
@@ -425,31 +426,29 @@ SB_DEVICE bool k1_finish(const uint8_t* win, uint32_t n, uint16_t* table, unsign
     }
     K1_TICK(5);                                                  // [5] commit + verify (+ clash handling)
     // ---- exit state and copy-end insert
+    // (warp-uniform values, written as selects: only the copy-end insert below is a branch)
     const uint32_t ncopy = popc(CS);
-    const unsigned last = ncopy ? 31 - clz(CS) : 0;
-    const uint32_t e_last = ncopy ? last + shfl(L, last) : 0;
-    if (ncopy && e_last >= 32) {
-        st.s = w + e_last; st.rematch = true;
-        if (e_last >= 33) {                                       // e-1 lies beyond this window
-            if (nxt->w == w + 32 && e_last <= 64) {
-                // ... but inside the next one, whose sequential words are already prefetched: take
-                // its hash from the lane that holds it instead of paying a global load (:293-295)
-                if (st.s < s_limit) {
-                    const unsigned nsh = (unsigned)((uintptr_t)(win + nxt->w + lane) & 3u) * 8;
-                    const uint32_t hsel = shfl(K1_HASH(funnel_r(nxt->a0, nxt->a1, nsh)), e_last - 33);
-                    syncwarp();
-                    if (lane == 0) table[hsel] = (uint16_t)(st.s - 1);
-                    syncwarp();
-                }
-            } else {
-                k1_preinsert(win, table, shift, s_limit, st.s);
+    const uint32_t e_last = reduce_max(taken ? lane + L : 0u);    // end of the window's last copy, 0 without one
+    const bool over = e_last >= 32;                               // that copy ends at or beyond the window's end
+    // else the window ends in a scan: probes since the last copy end, since the rematch miss at i0, or the running scan's
+    const uint32_t scan_skip = CS ? 32 + (31 - e_last) : st.rematch ? 32 + (31 - i0) : st.skip + (32 - i0);
+    st.s = w + (over ? e_last : 32);
+    st.skip = over ? st.skip : scan_skip;
+    st.rematch = over;
+    if (e_last >= 33) {                                       // e-1 lies beyond this window
+        if (nxt->w == w + 32 && e_last <= 64) {
+            // ... but inside the next one, whose sequential words are already prefetched: take
+            // its hash from the lane that holds it instead of paying a global load (:293-295)
+            if (st.s < s_limit) {
+                const unsigned nsh = (unsigned)((uintptr_t)(win + nxt->w + lane) & 3u) * 8;
+                const uint32_t hsel = shfl(K1_HASH(funnel_r(nxt->a0, nxt->a1, nsh)), e_last - 33);
+                syncwarp();
+                if (lane == 0) table[hsel] = (uint16_t)(st.s - 1);
+                syncwarp();
             }
+        } else {
+            k1_preinsert(win, table, shift, s_limit, st.s);
         }
-    } else if (ncopy) {
-        st.s = w + 32; st.rematch = false; st.skip = 32 + (31 - e_last);
-    } else {
-        st.skip = st.rematch ? 32 + (31 - i0) : st.skip + (32 - i0);
-        st.s = w + 32; st.rematch = false;
     }
     const uint32_t slot = popc(CS & ((1u << lane) - 1u));     // this lane's event among the window's copies
     K1_TICK(7);                                                  // [7] exit state / copy-end insert
