@@ -176,6 +176,29 @@ int sb_decompress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint
 uint64_t sb_compress_batch_scratch_bytes(uint32_t count, uint64_t in_bytes);
 int sb_compress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, void* scratch, uint64_t scratch_bytes,
                                 void* stream, sb_error* err);
+/* Frame encode of units of ANY length: unit i becomes exactly what sb_frame_encode(input_i) produces, that is
+ * `FrameEncoder::new(vec![]).write_all(input_i); into_inner()` (src/write.rs:123-192): the stream identifier, then one
+ * chunk per <= 65536-byte slice, compressed or stored by the reference's rule. The same addressing as the other batch
+ * calls; every chunk of every unit is compressed in one launch, then each unit is assembled in its output. Per unit, with
+ * n = in_len_i and cap_i = out_caps[i] or the uniform cap:
+ *   Ok: out_lens[i] = the stream's length; an empty unit writes nothing and has out_lens[i] = 0 (src/write.rs:155-157).
+ *   BufferTooSmall{given=cap_i, min=sb_frame_max_len(n)} when cap_i is smaller (so every n > 3,679,453,184).
+ *   A rejected unit has out_lens[i] = 0, and neither its input nor its output is touched. statuses may be NULL.
+ *   in_bytes: as for sb_compress_batch_device_ws, the caller's bound on the sum of in_lens over units of MORE than 65536
+ *     bytes; the scratch, sb_frame_encode_batch_scratch_bytes(count, in_bytes) bytes, depends on nothing else. When those
+ *     lengths sum to more than in_bytes on the device, every such unit gets SB_E_INVALID{a=sum, b=in_bytes} and
+ *     out_lens 0; units of at most 65536 bytes are still encoded.
+ *   d_chunk_offs: optional (device). Unit i's index starts at entry i + sum_{j<i} ceil(n_j / 65536) and holds
+ *     ceil(n_i / 65536) + 1 entries: the offset of every chunk header in the unit's output (the first is 10), then the
+ *     stream length -- the index sb_frame_encode_device_ws emits and sb_frame_decode_device_ws accepts. An empty unit
+ *     gets the single entry 0; a rejected unit's entries are not written.
+ * Stream ordered, no allocation, no host synchronisation; a unit's input and output must not overlap. Null pointers
+ * (batch, out_lens, scratch), count >= 2^31, a bound whose chunk count does not fit one launch
+ * (sb_frame_encode_batch_scratch_bytes returns UINT64_MAX) and scratch that is too small are SB_E_INVALID with nothing
+ * launched; count == 0 does nothing. Like sb_compress_batch_device, launches on different streams are ordered. */
+uint64_t sb_frame_encode_batch_scratch_bytes(uint32_t count, uint64_t in_bytes);
+int sb_frame_encode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint64_t* d_chunk_offs,
+                                    void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
 /* Masked CRC-32C of each unit (frame chunks): out_lens[i] receives the CRC. */
 int sb_crc32c_masked_batch_device(const sb_batch* batch, void* stream, sb_error* err);
 

@@ -41,12 +41,15 @@ SB_DEVICE uint32_t k4_chunk_len(uint64_t n, uint32_t i) {
     const uint64_t left = n - at;
     return left > kMaxBlock ? kMaxBlock : (uint32_t)left;
 }
+// a chunk of n input bytes that compresses to c bytes (varint included) is stored uncompressed (src/frame.rs:85).
+// A macro, not a function: K4's kernels then compile to the same code as with the comparison written out.
+#define K4_CHUNK_RAW(c, n) ((c) >= (n) - (n) / 8)
 // bytes chunk i occupies in the final stream
 SB_DEVICE uint32_t k4_chunk_size(const FramePlan& p, uint32_t i) {
     const uint32_t c = p.clens[i];
     if (!p.frame) return c;
     const uint32_t n = k4_chunk_len(p.n, i);
-    return 8 + ((c >= n - n / 8) ? n : c);                          // src/frame.rs:85
+    return 8 + (K4_CHUNK_RAW(c, n) ? n : c);
 }
 
 // per-chunk input lengths for K1: all 65536 except the last (src/write.rs:171-174)
@@ -134,7 +137,7 @@ SB_DEVICE void k4_gather_body(const FramePlan& p) {
         const uint8_t* slot = p.slots + (uint64_t)i * kSlotStride;
         if (p.frame) {
             const uint32_t n = k4_chunk_len(p.n, i), c = p.clens[i];
-            const bool raw = c >= n - n / 8;
+            const bool raw = K4_CHUNK_RAW(c, n);
             const uint32_t body = raw ? n : c, clen = 4 + body, crc = p.crcs[i];
             if (lane < 8) {
                 const uint64_t hdr = (uint64_t)(raw ? 1u : 0u) | ((uint64_t)clen << 8) | ((uint64_t)crc << 32);

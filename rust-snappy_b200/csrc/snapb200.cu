@@ -22,6 +22,7 @@
 #include "k7_frame_index.cuh"
 #include "k8_raw_split.cuh"
 #include "k9_raw_batch_compress.cuh"
+#include "k10_frame_batch_encode.cuh"
 
 namespace {
 
@@ -82,6 +83,13 @@ __global__ void __launch_bounds__(1024) k9_bscan_local_kernel(sbk::RawCompressPl
 __global__ void __launch_bounds__(1024) k9_bscan_tiles_kernel(sbk::RawCompressPlan q) { sbk::k9_bscan_tiles_body(q); }
 __global__ void __launch_bounds__(256) k9_gather_kernel(sbk::RawCompressPlan q) { sbk::k9_gather_body(q); }
 __global__ void __launch_bounds__(256) k9_finish_kernel(sbk::RawCompressPlan q) { sbk::k9_finish_body(q); }
+__global__ void __launch_bounds__(256) k10_plan_kernel(sbk::FrameBatchPlan q) { sbk::k10_plan_body(q); }
+__global__ void __launch_bounds__(1024) k10_iscan_local_kernel(sbk::FrameBatchPlan q) { sbk::k10_iscan_local_body(q); }
+__global__ void __launch_bounds__(1024) k10_iscan_tiles_kernel(sbk::FrameBatchPlan q) { sbk::k10_iscan_tiles_body(q); }
+__global__ void __launch_bounds__(256) k10_fill_kernel(sbk::FrameBatchPlan q) { sbk::k10_fill_body(q); }
+__global__ void __launch_bounds__(1024) k10_bscan_local_kernel(sbk::FrameBatchPlan q) { sbk::k10_bscan_local_body(q); }
+__global__ void __launch_bounds__(256) k10_gather_kernel(sbk::FrameBatchPlan q) { sbk::k10_gather_body(q); }
+__global__ void __launch_bounds__(256) k10_finish_kernel(sbk::FrameBatchPlan q) { sbk::k10_finish_body(q); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -573,6 +581,41 @@ int launch_raw_compress(Ctx& c, const sb_batch& b, uint64_t in_bytes, void* scra
     return 0;
 }
 
+// ---- frame batch encode (K9's plan and slots, K1 in frame mode, frame chunks assembled per unit)
+uint64_t frame_batch_ws_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k10_carve(nullptr, count, in_bytes, nullptr); }
+int launch_frame_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint64_t* d_chunk_offs, void* scratch, cudaStream_t st,
+                       sb_error* err) {
+    sbk::FrameBatchPlan q;
+    memset(&q, 0, sizeof q);
+    q.r.b = b; q.idx = d_chunk_offs;
+    sbk::k10_carve(scratch, b.count, in_bytes, &q);
+    auto threads = [](uint64_t n, unsigned per) { return (unsigned)((n + per - 1) / per); };
+    // warp-per-item kernels: 8 warps per CTA, at most 16 CTAs per SM, grid-stride beyond that
+    auto warps = [&](uint64_t n) { const uint64_t g = (n + 7) / 8, most = (uint64_t)16 * c.sms; return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most; };
+    CK(cudaMemsetAsync(q.r.ctl, 0, sizeof(sbk::RawCompressCtl), st));
+    k10_plan_kernel<<<threads(b.count, 256), 256, 0, st>>>(q);
+    k9_scan_local_kernel<<<threads((uint64_t)b.count + 1, sbk::K4_TILE), sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q.r);
+    k9_scan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q.r);
+    g_launches += 3;
+    if (d_chunk_offs) {
+        k10_iscan_local_kernel<<<threads((uint64_t)b.count + 1, sbk::K4_TILE), sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+        k10_iscan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+        g_launches += 2;
+    }
+    k10_fill_kernel<<<threads(q.r.nk, 256), 256, 0, st>>>(q);
+    g_launches++;
+    CK(cudaGetLastError());
+    int rc = launch_k1(c, sbk::k9_k1_batch(q.r), 1u, q.crcs, st, err);
+    if (rc) return rc;
+    k10_bscan_local_kernel<<<threads((uint64_t)q.r.nslot + 1, sbk::K4_TILE), sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k9_bscan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q.r);
+    k10_gather_kernel<<<warps(q.r.nslot), 256, 0, st>>>(q);
+    k10_finish_kernel<<<warps(b.count), 256, 0, st>>>(q);
+    g_launches += 4;
+    CK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 // =========================================================================
@@ -711,6 +754,25 @@ int sb_compress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, void* 
     int rc = get_ctx(&c, err);
     if (rc) return rc;
     rc = launch_raw_compress(*c, *batch, in_bytes, scratch, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_frame_encode_batch_scratch_bytes(uint32_t count, uint64_t in_bytes) { return frame_batch_ws_bytes(count, in_bytes); }
+
+int sb_frame_encode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint64_t* d_chunk_offs, void* scratch,
+                                    uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if (!batch || !batch->out_lens || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K9_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K9_MAX_COUNT);
+    if (batch->count == 0) { ok(err); return 0; }
+    const uint64_t need = frame_batch_ws_bytes(batch->count, in_bytes);
+    if (need == ~0ull) return fail(err, SB_E_INVALID, batch->count, in_bytes);   // more chunks than one K1 launch takes
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_frame_batch(*c, *batch, in_bytes, d_chunk_offs, scratch, (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;

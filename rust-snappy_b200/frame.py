@@ -27,6 +27,62 @@ def encode_chunks(data, include_ident: bool) -> bytes:
     return bytes(out[:m.value])
 
 
+def max_len(n: int) -> int:
+    """sb_frame_max_len(n): the identifier and the largest chunk per started 64 KB slice."""
+    return len(STREAM_IDENTIFIER) + (n + MAX_BLOCK_SIZE - 1) // MAX_BLOCK_SIZE * (CHUNK_HEADER_AND_CRC_SIZE +
+                                                                                   MAX_COMPRESS_BLOCK_SIZE)
+
+
+def encode_batch(units) -> list:
+    """Every unit as `FrameEncoder::new(vec![]).write_all(unit); into_inner()`, which is what sb_frame_encode returns: a
+    complete framed stream per unit, b"" for an empty one. Units are bytes-like (bytes, bytearray, memoryview, numpy
+    arrays). One sb_frame_encode_batch_device_ws call on the current torch stream encodes all of them; the inputs go to
+    the device in one copy and the streams come back in one. Raises the first failing unit's error."""
+    import numpy as np
+    import torch
+    L = _lib.lib()
+    views = [np.frombuffer(u, dtype=np.uint8) for u in units]
+    count = len(views)
+    if count == 0:
+        return []
+    lens = [v.size for v in views]
+    caps = [min(max_len(n), 0xFFFFFFFF) for n in lens]                # a longer unit is BufferTooSmall, never written
+    in_offs = np.zeros(count, dtype=np.int64)
+    in_offs[1:] = np.cumsum(lens[:-1])
+    host = np.empty(sum(lens) + 1, dtype=np.uint8)
+    for o, v in zip(in_offs, views):
+        host[o:o + v.size] = v
+    out_offs = np.zeros(count, dtype=np.int64)
+    room = [c if c == max_len(n) else 0 for n, c in zip(lens, caps)]
+    out_offs[1:] = np.cumsum(room[:-1])
+    # one device buffer holds the streams, then out_lens (u32) and the statuses (sb_error, 32 bytes), 8-byte aligned
+    at_lens = (sum(room) + 7) // 8 * 8
+    at_st = at_lens + (4 * count + 7) // 8 * 8
+    dev = torch.device("cuda", torch.cuda.current_device())
+    t_in = torch.from_numpy(host).to(dev)
+    t_out = torch.empty(at_st + 32 * count, dtype=torch.uint8, device=dev)
+    desc = np.concatenate([in_offs + t_in.data_ptr(), out_offs + t_out.data_ptr(),
+                           np.array(lens + caps, dtype=np.uint32).view(np.int64)])
+    t_desc = torch.from_numpy(desc).to(dev)
+    b = _lib.SbBatch()
+    b.in_ptrs, b.out_ptrs = t_desc.data_ptr(), t_desc.data_ptr() + 8 * count
+    b.in_lens, b.out_caps = t_desc.data_ptr() + 16 * count, t_desc.data_ptr() + 20 * count
+    b.out_lens, b.statuses, b.count = t_out.data_ptr() + at_lens, t_out.data_ptr() + at_st, count
+    in_bytes = sum(n for n, r in zip(lens, room) if n > MAX_BLOCK_SIZE and r)
+    need = L.sb_frame_encode_batch_scratch_bytes(count, in_bytes)
+    t_scr = torch.empty(need, dtype=torch.uint8, device=dev)
+    e = _lib.SbError()
+    if L.sb_frame_encode_batch_device_ws(C.byref(b), in_bytes, None, t_scr.data_ptr(), need,
+                                         torch.cuda.current_stream(dev).cuda_stream, C.byref(e)):
+        raise from_c(e)
+    back = t_out.cpu().numpy()
+    out_lens = back[at_lens:at_lens + 4 * count].view(np.uint32)
+    for st in back[at_st:].view(np.uint64).reshape(count, 4):
+        if st[0] & 0xFFFFFFFF:
+            raise from_c(_lib.SbError(int(st[0] & 0xFFFFFFFF), 0, int(st[1]), int(st[2]), int(st[3])))
+    return [back[o:o + k].tobytes() for o, k in zip(out_offs, out_lens)]
+
+
 def decode_all(stream) -> bytes:
     """read::FrameDecoder::new(stream).read_to_end() (src/read.rs:104-239)."""
     n = len(stream)
