@@ -199,6 +199,37 @@ int sb_compress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, void* 
 uint64_t sb_frame_encode_batch_scratch_bytes(uint32_t count, uint64_t in_bytes);
 int sb_frame_encode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint64_t* d_chunk_offs,
                                     void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
+/* Frame decode of a batch of streams: unit i is one frame stream, decoded as `FrameDecoder::new(unit_i).read_to_end()`
+ * (src/read.rs:104-239). statuses[i] and out_lens[i] equal the status and bytes sb_frame_decode_device_ws(unit_i, cap_i,
+ * ..., flags) writes to its sb_frame_result given a chunk table large enough, and out_i[0 .. out_lens[i]) equals that
+ * call's output: Ok with the decoded length, the reader's first error in stream order with the bytes produced before
+ * it, or BufferTooSmall{given=cap_i, min=decoded length} with nothing decoded. Beyond out_lens[i] a failing unit's
+ * output is unspecified; an empty unit is Ok with 0 bytes. The same addressing as the other batch calls; statuses and
+ * out_lens are required. Every unit's chunk index is built (or checked) in parallel and the chunks of all units are
+ * decoded side by side in one grid; a unit that is not a clean run of data chunks is walked by one thread.
+ *   flags bit0: no stream identifier expected, for every unit (fragments).
+ *   d_chunk_offs, d_index_at: optional caller index (device), both or neither. Unit i's is
+ *     d_chunk_offs[d_index_at[i] .. d_index_at[i+1]): the offset of every chunk header in the unit, then its length --
+ *     the layout sb_frame_encode_batch_device_ws writes, where d_index_at[i] = i + sum_{j<i} ceil(n_j / 65536). An
+ *     index that does not describe its unit costs speed, never a result: that unit is walked.
+ *   in_bytes: the caller's bound on the sum of in_lens; it sizes only the parallel indexer's tables. When the lengths sum
+ *     to more on the device, units without a caller index are walked: results stay exact. Bounds above 2^36 count as
+ *     2^36.
+ *   max_chunks: slots of the batch's chunk table, 1 .. 4,194,302. Units take ranges of data chunks in batch order; the
+ *     first unit whose chunks do not fit and every unit after it get SB_E_INVALID{a=max_chunks, b=1} (the single call's
+ *     "chunk table too small", with the same priority over BufferTooSmall) and out_lens 0. With a caller index the
+ *     exact need is d_index_at[count] - d_index_at[0] - count; n_i / 8 summed over the units is always enough.
+ *   d_unit_chunks: optional (device, count entries): the data chunks of unit i the parallel parse placed, 0 when one
+ *     thread walked the unit.
+ * Stream ordered, no allocation, no host synchronisation; the scratch, sb_frame_decode_batch_scratch_bytes(count,
+ * in_bytes, max_chunks) bytes, depends on nothing else and need not be zeroed. Null pointers (batch, out_lens, statuses,
+ * scratch), count >= 2^31, max_chunks == 0 or over the limit, an index given half and scratch that is too small are
+ * SB_E_INVALID with nothing launched; count == 0 does nothing. */
+uint64_t sb_frame_decode_batch_scratch_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks);
+int sb_frame_decode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t flags,
+                                    const uint64_t* d_chunk_offs, const uint64_t* d_index_at, uint32_t max_chunks,
+                                    uint32_t* d_unit_chunks, void* scratch, uint64_t scratch_bytes,
+                                    void* stream, sb_error* err);
 /* Masked CRC-32C of each unit (frame chunks): out_lens[i] receives the CRC. */
 int sb_crc32c_masked_batch_device(const sb_batch* batch, void* stream, sb_error* err);
 

@@ -60,6 +60,32 @@ SB_DEVICE uint32_t k5_varint(const uint8_t* p, uint32_t n, uint64_t* out) {
     return 0;
 }
 
+// The chunk whose header is at `at` of in[0..n), given the next header at `next` (an index entry pair): a data chunk
+// (type 0/1, 4 <= len <= 76490, a stored body of at most 65536 bytes, a varint of at most 65536 within the body's first
+// 10 bytes) that ends exactly at `next`. *c = its record; false for anything else (the caller walks the stream).
+SB_DEVICE bool k5_check_chunk(const uint8_t* in, uint64_t n, uint64_t at, uint64_t next, FChunk* c) {
+    bool ok = at + 8 <= n && next > at && next <= n;
+    c->body_off = 0; c->body_len = 0; c->dlen = 0; c->want_crc = 0; c->type = 0;
+    if (ok) {
+        const uint8_t* h = in + at;
+        const uint32_t ty = h[0], len = (uint32_t)h[1] | ((uint32_t)h[2] << 8) | ((uint32_t)h[3] << 16);
+        ok = (ty == 0 || ty == 1) && len >= 4 && len <= K5_MAX_CBLOCK && at + 4 + len == next;
+        if (ok) {
+            c->type = ty;
+            c->want_crc = (uint32_t)h[4] | ((uint32_t)h[5] << 8) | ((uint32_t)h[6] << 16) | ((uint32_t)h[7] << 24);
+            c->body_off = at + 8; c->body_len = len - 4;
+            if (ty == 1) { ok = c->body_len <= kMaxBlock; c->dlen = c->body_len; }
+            else {
+                uint64_t v = 0;
+                const uint32_t hl = k5_varint(h + 8, c->body_len < 10 ? c->body_len : 10, &v);
+                ok = hl != 0 && v <= kMaxBlock;
+                c->dlen = (uint32_t)v;
+            }
+        }
+    }
+    return ok;
+}
+
 // ---- parallel header parse over a caller-provided chunk index (clean streams only; anything else -> need_serial)
 SB_DEVICE void k5_parse_body(const DecodePlan& p) {
     const uint64_t i = (uint64_t)block_idx() * block_dim() + thread_idx();
@@ -81,45 +107,26 @@ SB_DEVICE void k5_parse_body(const DecodePlan& p) {
         ctl->nchunks = index_n <= p.cap_chunks ? index_n : 0;
     }
     if (i >= index_n || i >= p.cap_chunks) return;
-    const uint64_t at = p.index[i], next = p.index[i + 1];
-    bool ok = at + 8 <= p.n && next > at && next <= p.n;
     FChunk c;
-    c.body_off = 0; c.body_len = 0; c.dlen = 0; c.want_crc = 0; c.type = 0;
-    if (ok) {
-        const uint8_t* h = p.in + at;
-        const uint32_t ty = h[0], len = (uint32_t)h[1] | ((uint32_t)h[2] << 8) | ((uint32_t)h[3] << 16);
-        ok = (ty == 0 || ty == 1) && len >= 4 && len <= K5_MAX_CBLOCK && at + 4 + len == next;
-        if (ok) {
-            c.type = ty;
-            c.want_crc = (uint32_t)h[4] | ((uint32_t)h[5] << 8) | ((uint32_t)h[6] << 16) | ((uint32_t)h[7] << 24);
-            c.body_off = at + 8; c.body_len = len - 4;
-            if (ty == 1) { ok = c.body_len <= kMaxBlock; c.dlen = c.body_len; }
-            else {
-                uint64_t v = 0;
-                const uint32_t hl = k5_varint(h + 8, c.body_len < 10 ? c.body_len : 10, &v);
-                ok = hl != 0 && v <= kMaxBlock;
-                c.dlen = (uint32_t)v;
-            }
-        }
-    }
-    if (!ok) { ctl->need_serial = 1; c.dlen = 0; }
+    if (!k5_check_chunk(p.in, p.n, p.index[i], p.index[i + 1], &c)) { ctl->need_serial = 1; c.dlen = 0; }
     p.chunks[i] = c;
 }
 
-// ---- serial walk, thread 0 of one warp: exactly the reader's control flow (src/read.rs:111-237)
-SB_DEVICE void k5_walk_body(const DecodePlan& p) {
-    DecodeCtl* ctl = p.ctl;
-    if (thread_idx() != 0 || block_idx() != 0) return;
-    if (p.index && !ctl->need_serial) return;                        // the parallel parse was enough
-    const uint8_t* in = p.in;
-    const uint64_t n = p.n;
+// ---- serial walk of in[0..n) by one thread: exactly the reader's control flow (src/read.rs:111-237), including its
+// quirk that decompress_len() sees the persistent source buffer (src/read.rs:216). Every data chunk up to the first
+// error goes to sink(i, chunk), at most cap_chunks of them (then SB_E_INVALID{cap_chunks, 1}: chunk table too small).
+// Returns the chunk count; *err = the reader's first error (or Ok), *out_produced = the chunks' decompressed bytes.
+// Every chunk type advances pos by 4 + its length, so the walk visits a prefix of the stream's header chain.
+template <class Sink>
+SB_DEVICE uint32_t k5_walk(const uint8_t* in, uint64_t n, bool fragment, uint32_t cap_chunks, Sink sink, sb_error* err,
+                           uint64_t* out_produced) {
     uint8_t shadow[16];                                              // first bytes of the reader's persistent `src` buffer
     for (int k = 0; k < 16; k++) shadow[k] = 0;
     sb_error werr;
     k5_set(&werr, SB_OK);
     uint64_t pos = 0, produced = 0;
     uint32_t count = 0;
-    bool seen_ident = p.fragment != 0;
+    bool seen_ident = fragment;
     while (pos < n) {
         if (n - pos < 4) { k5_set(&werr, SB_IO_UNEXPECTED_EOF); break; }
         const uint8_t* h = in + pos;
@@ -172,12 +179,26 @@ SB_DEVICE void k5_walk_body(const DecodePlan& p) {
                 for (uint32_t k = 0; k < fresh; k++) shadow[k] = in[pos + k];
             }
             pos += body;
-            if (count >= p.cap_chunks) { k5_set(&werr, SB_E_INVALID, p.cap_chunks, 1); break; }   // chunk table too small
-            p.chunks[count++] = c;
+            if (count >= cap_chunks) { k5_set(&werr, SB_E_INVALID, cap_chunks, 1); break; }   // chunk table too small
+            sink(count++, c);
             produced += c.dlen;
         }
     }
-    ctl->nchunks = count;
+    *err = werr;
+    *out_produced = produced;
+    return count;
+}
+
+// thread 0 of one warp
+SB_DEVICE void k5_walk_body(const DecodePlan& p) {
+    DecodeCtl* ctl = p.ctl;
+    if (thread_idx() != 0 || block_idx() != 0) return;
+    if (p.index && !ctl->need_serial) return;                        // the parallel parse was enough
+    FChunk* chunks = p.chunks;
+    sb_error werr;
+    uint64_t produced;
+    ctl->nchunks = k5_walk(p.in, p.n, p.fragment != 0, p.cap_chunks, [&](uint32_t i, const FChunk& c) { chunks[i] = c; },
+                           &werr, &produced);
     ctl->walk_err = werr;
     ctl->produced = produced;                                         // provisional (the scan recomputes it)
 }
@@ -199,6 +220,21 @@ SB_DEVICE void k5_scan_tiles_body(const DecodePlan& p) {
     }
 }
 
+// One chunk by the calling warp: K2 decode or plain copy of its body to dst, then the masked CRC-32C of the produced
+// bytes against the header's (Error::Checksum, src/read.rs:189-196 / :226-233). *st = the chunk's status; returns its code.
+SB_DEVICE uint32_t k5_decode_chunk(const uint32_t* tab, uint32_t* elems, const FChunk& c, const uint8_t* in, uint8_t* dst,
+                                   sb_error* st) {
+    uint32_t code = SB_OK;
+    if (c.type == 0) code = k2_decode_stream(in + c.body_off, c.body_len, dst, c.dlen, st, nullptr, elems);
+    else { warp_copy(dst, in + c.body_off, c.body_len); if (lane_id() == 0) k5_set(st, SB_OK); }
+    syncwarp();
+    if (code == SB_OK) {
+        const uint32_t got = k3_warp_crc32c_masked(tab, dst, c.dlen);
+        if (got != c.want_crc) { code = SB_CHECKSUM; if (lane_id() == 0) k5_set(st, SB_CHECKSUM, c.want_crc, got); }
+    }
+    return code;
+}
+
 // warp per chunk: decode / copy, then verify the checksum while the output is hot in L2
 SB_DEVICE void k5_decode_body(const DecodePlan& p) {
     uint32_t* tab = (uint32_t*)smem();                                // K3 slicing tables (4 KB)
@@ -213,15 +249,7 @@ SB_DEVICE void k5_decode_body(const DecodePlan& p) {
         const FChunk c = p.chunks[u];
         const uint64_t off = p.tiles[u / K4_TILE] + p.ooff[u];
         uint8_t* dst = p.out + off;
-        sb_error* st = &p.statuses[u];
-        uint32_t code = SB_OK;
-        if (c.type == 0) code = k2_decode_stream(p.in + c.body_off, c.body_len, dst, c.dlen, st, nullptr, elems);
-        else { warp_copy(dst, p.in + c.body_off, c.body_len); if (lane == 0) k5_set(st, SB_OK); }
-        syncwarp();
-        if (code == SB_OK) {
-            const uint32_t got = k3_warp_crc32c_masked(tab, dst, c.dlen);
-            if (got != c.want_crc) { code = SB_CHECKSUM; if (lane == 0) k5_set(st, SB_CHECKSUM, c.want_crc, got); }
-        }
+        const uint32_t code = k5_decode_chunk(tab, elems, c, p.in, dst, &p.statuses[u]);
         if (code != SB_OK && lane == 0) atomic_min(&p.ctl->first_bad, (uint32_t)u);
         syncwarp();
         if (lane == 0) p.ooff[u] = off;                                 // absolute from here on

@@ -97,9 +97,8 @@ SB_DEVICE bool k7_hop(const uint8_t* in, uint64_t n, uint64_t p, uint64_t* next)
     return true;
 }
 
-SB_DEVICE void k7_survivors_body(const IndexPlan& p) {
-    const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
-    if (p.decline || k >= p.nseg) return;
+// segment k < p.nseg of a stream that is not declined, by the calling warp
+SB_DEVICE void k7_survivors_seg(const IndexPlan& p, uint64_t k) {
     const unsigned lane = lane_id();
     const uint8_t* in = p.in;
     const uint64_t n = p.n, b = p.s0 + k * p.seg;
@@ -137,6 +136,11 @@ SB_DEVICE void k7_survivors_body(const IndexPlan& p) {
         }
     }
     if (lane == 0) p.nsurv[k] = kept < K7_KEEP ? kept : K7_KEEP;
+}
+SB_DEVICE void k7_survivors_body(const IndexPlan& p) {
+    const uint64_t k = (uint64_t)block_idx() * (block_dim() >> 5) + warp_id();
+    if (p.decline || k >= p.nseg) return;
+    k7_survivors_seg(p, k);
 }
 
 SB_DEVICE void k7_stitch_body(const IndexPlan& p) {
@@ -188,12 +192,8 @@ SB_DEVICE void k7_stitch_body(const IndexPlan& p) {
     if (t == 0) *p.count = ok && e == p.n ? (uint32_t)total : (uint32_t)SB_FRAME_NOT_INDEXABLE;
 }
 
-SB_DEVICE void k7_emit_body(const IndexPlan& p) {
-    const uint64_t k = (uint64_t)block_idx() * block_dim() + thread_idx();
-    const uint32_t total = *p.count;
-    if (total == SB_FRAME_NOT_INDEXABLE) return;
-    if (k == 0) p.index[total] = p.n;
-    if (k >= p.nseg) return;
+// the index entries of the chunks of segment k < p.nseg of an indexed stream
+SB_DEVICE void k7_emit_seg(const IndexPlan& p, uint64_t k) {
     const uint64_t b = p.s0 + k * p.seg;
     const uint64_t lim = b + p.seg < p.n ? b + p.seg : p.n;
     uint64_t at = b + p.ent[k];
@@ -202,6 +202,14 @@ SB_DEVICE void k7_emit_body(const IndexPlan& p) {
         p.index[j++] = at;
         at += 4 + ((uint32_t)p.in[at + 1] | ((uint32_t)p.in[at + 2] << 8) | ((uint32_t)p.in[at + 3] << 16));
     }
+}
+SB_DEVICE void k7_emit_body(const IndexPlan& p) {
+    const uint64_t k = (uint64_t)block_idx() * block_dim() + thread_idx();
+    const uint32_t total = *p.count;
+    if (total == SB_FRAME_NOT_INDEXABLE) return;
+    if (k == 0) p.index[total] = p.n;
+    if (k >= p.nseg) return;
+    k7_emit_seg(p, k);
 }
 
 }  // namespace sbk

@@ -23,6 +23,7 @@
 #include "k8_raw_split.cuh"
 #include "k9_raw_batch_compress.cuh"
 #include "k10_frame_batch_encode.cuh"
+#include "k11_frame_batch_decode.cuh"
 
 namespace {
 
@@ -90,6 +91,20 @@ __global__ void __launch_bounds__(256) k10_fill_kernel(sbk::FrameBatchPlan q) { 
 __global__ void __launch_bounds__(1024) k10_bscan_local_kernel(sbk::FrameBatchPlan q) { sbk::k10_bscan_local_body(q); }
 __global__ void __launch_bounds__(256) k10_gather_kernel(sbk::FrameBatchPlan q) { sbk::k10_gather_body(q); }
 __global__ void __launch_bounds__(256) k10_finish_kernel(sbk::FrameBatchPlan q) { sbk::k10_finish_body(q); }
+__global__ void __launch_bounds__(1024) k11_plan_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_plan_body(q); }
+__global__ void __launch_bounds__(1024) k11_plan_tiles_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_plan_tiles_body(q); }
+__global__ void __launch_bounds__(128) k11_survivors_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_survivors_body(q); }
+__global__ void __launch_bounds__(sbk::K7_STITCH_THREADS) k11_stitch_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_stitch_body(q); }
+__global__ void __launch_bounds__(256) k11_link_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_link_body(q); }
+__global__ void __launch_bounds__(1024) k11_count_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_count_body(q); }
+__global__ void __launch_bounds__(1024) k11_range_tiles_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_range_tiles_body(q); }
+__global__ void __launch_bounds__(128) k11_emit_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_emit_body(q); }
+__global__ void __launch_bounds__(256) k11_parse_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_parse_body(q); }
+__global__ void __launch_bounds__(64) k11_fill_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_fill_body(q); }
+__global__ void __launch_bounds__(1024) k11_oscan_local_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_oscan_local_body(q); }
+__global__ void __launch_bounds__(1024) k11_oscan_tiles_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_oscan_tiles_body(q); }
+__global__ void __launch_bounds__(128) k11_decode_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_decode_body(q); }
+__global__ void __launch_bounds__(256) k11_finish_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_finish_body(q); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -616,6 +631,56 @@ int launch_frame_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint64_t* d
     return 0;
 }
 
+// ---- frame batch decode (K7's index or a walk per unit, K5's parse, decode and CRC over all units' chunks)
+uint64_t frame_decode_batch_ws_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks) {
+    return sbk::k11_carve(nullptr, count, in_bytes, max_chunks, nullptr);
+}
+int launch_frame_decode_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t flags, const uint64_t* d_chunk_offs,
+                              const uint64_t* d_index_at, uint32_t max_chunks, uint32_t* d_unit_chunks, void* scratch,
+                              cudaStream_t st, sb_error* err) {
+    sbk::FrameDecodeBatchPlan q;
+    memset(&q, 0, sizeof q);
+    q.b = b; q.fragment = flags & 1u; q.cidx = d_chunk_offs; q.cidx_at = d_index_at; q.unit_chunks = d_unit_chunks;
+    const uint64_t want = k7_want_seg();
+    q.seg = want < sbk::K7_SEG_MIN ? sbk::K7_SEG_MIN : want > (1ull << 31) ? (1ull << 31) : want;
+    sbk::k11_carve(scratch, b.count, in_bytes, max_chunks, &q);
+    // grids over lists whose true lengths are on the device: at most `per_sm` CTAs per SM, grid-stride beyond that
+    auto grid = [&](uint64_t items, unsigned per_cta, unsigned per_sm) {
+        const uint64_t g = (items + per_cta - 1) / per_cta, most = (uint64_t)per_sm * c.sms;
+        return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most;
+    };
+    const unsigned utiles = (unsigned)(((uint64_t)b.count + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    const unsigned stiles = (unsigned)(((uint64_t)max_chunks + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    CK(cudaMemsetAsync(q.in_total, 0, sizeof *q.in_total, st));
+    k11_plan_kernel<<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k11_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    if (d_chunk_offs) {
+        k11_link_kernel<<<grid((uint64_t)max_chunks + b.count, 256, 16), 256, 0, st>>>(q);
+        g_launches += 3;
+    } else {
+        k11_survivors_kernel<<<grid(q.nseg_cap, 4, 16), 128, 0, st>>>(q);
+        k11_stitch_kernel<<<b.count < (uint32_t)(8 * c.sms) ? b.count : (unsigned)(8 * c.sms), sbk::K7_STITCH_THREADS,
+                            sbk::K7_STITCH_SMEM, st>>>(q);
+        g_launches += 4;
+    }
+    k11_count_kernel<<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k11_range_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    g_launches += 2;
+    if (!d_chunk_offs) {
+        k11_emit_kernel<<<grid(q.nseg_cap, 128, 16), 128, 0, st>>>(q);
+        g_launches++;
+    }
+    k11_parse_kernel<<<grid(max_chunks, 256, 16), 256, 0, st>>>(q);
+    k11_fill_kernel<<<grid(b.count, 64, 32), 64, 0, st>>>(q);
+    k11_oscan_local_kernel<<<stiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k11_oscan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    k11_decode_kernel<<<grid(max_chunks, 4, 16), 128, sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    k11_finish_kernel<<<grid(b.count, 256, 16), 256, 0, st>>>(q);
+    g_launches += 6;
+    CK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 // =========================================================================
@@ -773,6 +838,30 @@ int sb_frame_encode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, ui
     int rc = get_ctx(&c, err);
     if (rc) return rc;
     rc = launch_frame_batch(*c, *batch, in_bytes, d_chunk_offs, scratch, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_frame_decode_batch_scratch_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks) {
+    return frame_decode_batch_ws_bytes(count, in_bytes, max_chunks);
+}
+
+int sb_frame_decode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t flags, const uint64_t* d_chunk_offs,
+                                    const uint64_t* d_index_at, uint32_t max_chunks, uint32_t* d_unit_chunks, void* scratch,
+                                    uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if (!batch || !batch->out_lens || !batch->statuses || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K11_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K11_MAX_COUNT);
+    if (!d_chunk_offs != !d_index_at) return fail(err, SB_E_INVALID);
+    if (max_chunks == 0 || max_chunks > sbk::K11_MAX_CHUNKS) return fail(err, SB_E_INVALID, max_chunks, sbk::K11_MAX_CHUNKS);
+    if (batch->count == 0) { ok(err); return 0; }
+    const uint64_t need = frame_decode_batch_ws_bytes(batch->count, in_bytes, max_chunks);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_frame_decode_batch(*c, *batch, in_bytes, flags, d_chunk_offs, d_index_at, max_chunks, d_unit_chunks, scratch,
+                                   (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;

@@ -83,6 +83,69 @@ def encode_batch(units) -> list:
     return [back[o:o + k].tobytes() for o, k in zip(out_offs, out_lens)]
 
 
+MAX_BATCH_CHUNKS = (1 << 22) - 2             # the largest chunk table sb_frame_decode_batch_device_ws takes
+
+
+def decode_batch(streams) -> list:
+    """Every stream as `FrameDecoder::new(stream).read_to_end()`: one bytes object per stream, b"" for an empty one.
+    Streams are bytes-like. The inputs go to the device in one copy and the decoded bytes come back in one; two
+    sb_frame_decode_batch_device_ws calls on the current torch stream do the work: one with every cap 0, whose
+    BufferTooSmall{0, need} sizes the outputs, then the decode. Raises the first failing stream's error."""
+    import numpy as np
+    import torch
+    L = _lib.lib()
+    views = [np.frombuffer(s, dtype=np.uint8) for s in streams]
+    count = len(views)
+    if count == 0:
+        return []
+    lens = [v.size for v in views]
+    in_offs = np.zeros(count, dtype=np.int64)
+    in_offs[1:] = np.cumsum(lens[:-1])
+    host = np.empty(sum(lens) + 1, dtype=np.uint8)
+    for o, v in zip(in_offs, views):
+        host[o:o + v.size] = v
+    dev = torch.device("cuda", torch.cuda.current_device())
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    t_in = torch.from_numpy(host).to(dev)
+    # out_lens (u32) and the statuses (sb_error, 32 bytes) of both calls, 8-byte aligned
+    at_st = (4 * count + 7) // 8 * 8
+    t_res = torch.empty(at_st + 32 * count, dtype=torch.uint8, device=dev)
+    e = _lib.SbError()
+
+    def call(out_offs, caps, out_base, max_chunks):
+        desc = np.concatenate([in_offs + t_in.data_ptr(), out_offs + out_base,
+                               np.array(lens + caps, dtype=np.uint32).view(np.int64)])
+        t_desc = torch.from_numpy(desc).to(dev)
+        b = _lib.SbBatch()
+        b.in_ptrs, b.out_ptrs = t_desc.data_ptr(), t_desc.data_ptr() + 8 * count
+        b.in_lens, b.out_caps = t_desc.data_ptr() + 16 * count, t_desc.data_ptr() + 20 * count
+        b.out_lens, b.statuses, b.count = t_res.data_ptr(), t_res.data_ptr() + at_st, count
+        need = L.sb_frame_decode_batch_scratch_bytes(count, sum(lens), max_chunks)
+        t_scr = torch.empty(need, dtype=torch.uint8, device=dev)
+        if L.sb_frame_decode_batch_device_ws(C.byref(b), sum(lens), 0, None, None, max_chunks, None, t_scr.data_ptr(),
+                                             need, stream, C.byref(e)):
+            raise from_c(e)
+        return t_res.cpu().numpy()[at_st:].view(np.uint64).reshape(count, 4)
+
+    zeros = np.zeros(count, dtype=np.int64)
+    # the chunk table: a data chunk is at least 8 bytes, so n / 8 per stream always suffices
+    max_chunks = min(sum(n // 1024 + 2 for n in lens), MAX_BATCH_CHUNKS)
+    st = call(zeros, [0] * count, t_in.data_ptr(), max_chunks)
+    if any(int(s[0]) & 0xFFFFFFFF == 202 and int(s[2]) == 1 for s in st):
+        max_chunks = min(sum(n // 8 + 2 for n in lens), MAX_BATCH_CHUNKS)
+        st = call(zeros, [0] * count, t_in.data_ptr(), max_chunks)
+    caps = [int(s[2]) if int(s[0]) & 0xFFFFFFFF == 2 else 0 for s in st]   # BufferTooSmall{0, need}
+    out_offs = np.zeros(count, dtype=np.int64)
+    out_offs[1:] = np.cumsum(caps[:-1])
+    t_out = torch.empty(sum(caps) + 1, dtype=torch.uint8, device=dev)
+    st = call(out_offs, caps, t_out.data_ptr(), max_chunks)
+    for s in st:
+        if s[0] & 0xFFFFFFFF:
+            raise from_c(_lib.SbError(int(s[0] & 0xFFFFFFFF), 0, int(s[1]), int(s[2]), int(s[3])))
+    back = t_out.cpu().numpy()
+    return [back[o:o + k].tobytes() for o, k in zip(out_offs, caps)]
+
+
 def decode_all(stream) -> bytes:
     """read::FrameDecoder::new(stream).read_to_end() (src/read.rs:104-239)."""
     n = len(stream)
