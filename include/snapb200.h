@@ -289,6 +289,37 @@ int sb_frame_decode_device_ws(const uint8_t* d_in, uint64_t n, uint8_t* d_out, u
 int sb_frame_decode_device(const uint8_t* d_in, uint64_t n, uint8_t* d_out, uint64_t cap,
                            const uint64_t* d_chunk_offs, uint32_t nchunks, uint32_t flags,
                            sb_frame_result* result, void* stream, sb_error* err);
+/* Byte ranges of one frame stream in device memory: range r receives decoded bytes [d_lo[r], d_lo[r] + d_len[r]) in
+ * d_out_ptrs[r] (device, d_len[r] bytes). Only the chunks a range covers are decoded and checksummed, so a window of a
+ * stream far larger than device memory costs its own chunks and one pass over the headers. The index phase is
+ * sb_frame_decode_device_ws's (d_chunk_offs/nchunks and flags bit0 work as there) and runs once per call.
+ *   Ranges may be empty, unsorted, overlapping, duplicated, or reach past the end; output buffers must not overlap each
+ *   other or the input. With end = min(lo + len, total), range r verifies chunk k (output offset off_k, decoded length
+ *   dlen_k) iff off_k < end && off_k + max(dlen_k, 1) > lo: the chunks producing its bytes and the empty chunks inside
+ *   it. Each verified chunk is decoded and its masked CRC-32C checked. d_statuses[r] and d_out_lens[r], in priority order:
+ *     1. chunk table too small: SB_E_INVALID{a=max_chunks, b=1}, 0;
+ *     2. a verified chunk fails: the first in stream order, k*, with its own status; max(off_k*, lo) - lo;
+ *     3. the range reaches past total and the header walk stopped on an error: that error; max(end - lo, 0);
+ *     4. otherwise Ok; max(end - lo, 0) (a range past a clean end is a short read, like pread).
+ *   out[0 .. out_len) is exactly what FrameDecoder::new(stream).read_to_end() gives for those bytes when every chunk the
+ *   range does not verify is valid; beyond it the bytes are unspecified. Nothing outside [out_r, out_r + max(end - lo,
+ *   0)) is written, so a buffer may hold just the bytes the stream can give the range. For a stream
+ *   sb_frame_decode_device_ws decodes Ok, every range is Ok and equals that output's slice.
+ *   *d_result: the stream's walk status (Invalid{max_chunks, 1}, the walk's stopping error, or Ok), bytes = total (the
+ *   decoded length of the chunks in the table) and nchunks. nranges == 0 writes only *d_result: the decoded length
+ *   without decoding.
+ *   max_chunks: chunk table slots, 1 .. 4,194,302.
+ * A chunk shared by several ranges is decoded once per range, and the scratch,
+ * sb_frame_decode_ranges_scratch_bytes(max_chunks, nranges) bytes, holds 128 KiB of staging per range for the chunks that
+ * straddle a range's ends; split very many small ranges over several calls. Stream ordered, no allocation, no host
+ * synchronisation, and the same number of launches whatever nranges. Null pointers that are needed, nranges >= 2^31,
+ * max_chunks out of range, nchunks > max_chunks with an index and scratch that is too small are SB_E_INVALID with
+ * nothing launched. */
+uint64_t sb_frame_decode_ranges_scratch_bytes(uint32_t max_chunks, uint32_t nranges);
+int sb_frame_decode_ranges_device_ws(const uint8_t* d_in, uint64_t n, const uint64_t* d_chunk_offs, uint32_t nchunks,
+                                     uint32_t flags, const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                                     uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, sb_frame_result* d_result,
+                                     void* scratch, uint64_t scratch_bytes, uint32_t max_chunks, void* stream, sb_error* err);
 
 /* Chunk index of a frame stream in device memory, built in parallel on the device:
  * the offset of every chunk header in d_in[0..n) followed by n -- exactly the

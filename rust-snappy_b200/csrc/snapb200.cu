@@ -24,6 +24,7 @@
 #include "k9_raw_batch_compress.cuh"
 #include "k10_frame_batch_encode.cuh"
 #include "k11_frame_batch_decode.cuh"
+#include "k12_frame_range_decode.cuh"
 
 namespace {
 
@@ -105,6 +106,11 @@ __global__ void __launch_bounds__(1024) k11_oscan_local_kernel(sbk::FrameDecodeB
 __global__ void __launch_bounds__(1024) k11_oscan_tiles_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_oscan_tiles_body(q); }
 __global__ void __launch_bounds__(128) k11_decode_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_decode_body(q); }
 __global__ void __launch_bounds__(256) k11_finish_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_finish_body(q); }
+__global__ void __launch_bounds__(1024) k12_plan_kernel(sbk::RangePlan q) { sbk::k12_plan_body(q); }
+__global__ void __launch_bounds__(1024) k12_plan_tiles_kernel(sbk::RangePlan q) { sbk::k12_plan_tiles_body(q); }
+// with the occupancy hint ptxas keeps the pair lookup in registers across K5's decode (without it: 64 and a 4-byte spill)
+__global__ void __launch_bounds__(128, 4) k12_decode_kernel(sbk::RangePlan q) { sbk::k12_decode_body(q); }
+__global__ void __launch_bounds__(256) k12_finish_kernel(sbk::RangePlan q) { sbk::k12_finish_body(q); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -681,6 +687,35 @@ int launch_frame_decode_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint
     return 0;
 }
 
+// ---- frame range decode (K5's index phase, then only the chunks the ranges cover: K12)
+uint64_t frame_range_ws_bytes(uint32_t max_chunks, uint32_t nranges) {
+    return decode_ws_bytes(max_chunks) + sbk::k12_carve(nullptr, nranges, nullptr);
+}
+int launch_frame_range_decode(Ctx& c, const uint8_t* d_in, uint64_t n, const uint64_t* d_chunk_offs, uint32_t nchunks,
+                              uint32_t flags, const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                              uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, sb_frame_result* d_result,
+                              void* scratch, uint32_t max_chunks, cudaStream_t st, sb_error* err) {
+    sbk::RangePlan q;
+    memset(&q, 0, sizeof q);
+    q.d = make_decode_plan(d_in, n, nullptr, ~0ull, d_chunk_offs, nchunks, (int)(flags & 1u), d_result, scratch, max_chunks);
+    q.lo = d_lo; q.len = d_len; q.outs = d_out_ptrs; q.out_lens = d_out_lens; q.statuses = d_statuses;
+    sbk::k12_carve((uint8_t*)scratch + decode_ws_bytes(max_chunks), nranges, &q);
+    int rc = decode_index_phase(c, q.d, st, err);
+    if (rc) return rc;
+    // the pair total is on the device: at most nranges * max_chunks pairs, 4 warps per CTA, at most 16 CTAs per SM
+    const uint64_t most = (uint64_t)16 * c.sms, pw = ((uint64_t)nranges * max_chunks + 3) / 4;
+    const unsigned ptiles = (unsigned)(((uint64_t)nranges + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    const uint64_t fg = ((uint64_t)nranges + 255) / 256;
+    k12_plan_kernel<<<ptiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k12_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    k12_decode_kernel<<<pw == 0 ? 1u : pw < most ? (unsigned)pw : (unsigned)most, 128,
+                        sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    k12_finish_kernel<<<fg == 0 ? 1u : fg < most ? (unsigned)fg : (unsigned)most, 256, 0, st>>>(q);
+    g_launches += 4;
+    CK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 // =========================================================================
@@ -862,6 +897,31 @@ int sb_frame_decode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, ui
     if (rc) return rc;
     rc = launch_frame_decode_batch(*c, *batch, in_bytes, flags, d_chunk_offs, d_index_at, max_chunks, d_unit_chunks, scratch,
                                    (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_frame_decode_ranges_scratch_bytes(uint32_t max_chunks, uint32_t nranges) {
+    return frame_range_ws_bytes(max_chunks, nranges);
+}
+
+int sb_frame_decode_ranges_device_ws(const uint8_t* d_in, uint64_t n, const uint64_t* d_chunk_offs, uint32_t nchunks,
+                                     uint32_t flags, const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                                     uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, sb_frame_result* d_result,
+                                     void* scratch, uint64_t scratch_bytes, uint32_t max_chunks, void* stream, sb_error* err) {
+    if ((!d_in && n) || !d_result || !scratch) return fail(err, SB_E_INVALID);
+    if (nranges && (!d_lo || !d_len || !d_out_ptrs || !d_out_lens || !d_statuses)) return fail(err, SB_E_INVALID);
+    if (nranges >= sbk::K12_MAX_RANGES) return fail(err, SB_E_INVALID, nranges, sbk::K12_MAX_RANGES);
+    if (max_chunks == 0 || max_chunks > sbk::K12_MAX_CHUNKS) return fail(err, SB_E_INVALID, max_chunks, sbk::K12_MAX_CHUNKS);
+    if (d_chunk_offs && nchunks > max_chunks) return fail(err, SB_E_INVALID, nchunks, max_chunks);
+    const uint64_t need = frame_range_ws_bytes(max_chunks, nranges);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_frame_range_decode(*c, d_in, n, d_chunk_offs, nchunks, flags, d_lo, d_len, d_out_ptrs, d_out_lens, d_statuses,
+                                   nranges, d_result, scratch, max_chunks, (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;

@@ -174,3 +174,116 @@ def decode_all_partial(stream):
     op, k2 = _ptr(out)
     rc = L.sb_frame_decode(ip, n, op, m.value, C.byref(m), C.byref(e))
     return bytes(out[:m.value]), (from_c(e) if rc else None)
+
+
+class RangeReader:
+    """Random access to the decoded bytes of one frame stream on the device: `read(lo, n)` returns decoded bytes
+    [lo, lo + n) as `FrameDecoder::new(stream).read_to_end()` would, after decoding and checksumming only the chunks
+    those bytes come from. A range past the end is a short read, like `pread`. The stream is a bytes-like object
+    (uploaded once) or a CUDA uint8 tensor (used as it is, and kept alive). It is indexed once on the device; a stream the
+    indexer declines (padding or skippable chunks, a repeated identifier, ...) is walked by one thread on every call.
+    fragment: the stream has no identifier. Calls run on the current torch stream and wait for their results."""
+
+    RANGES_PER_CALL = 4096                    # 128 KiB of staging per range: 512 MiB per call at most
+    BYTES_PER_CALL = 1 << 30                  # output bytes one call gathers (a single larger range gets its own call)
+
+    def __init__(self, stream, fragment=False):
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        self._dev = torch.device("cuda", torch.cuda.current_device())
+        if isinstance(stream, torch.Tensor):
+            if not stream.is_cuda or stream.dtype != torch.uint8 or stream.dim() != 1 or not stream.is_contiguous():
+                raise ValueError("RangeReader takes a contiguous 1-D CUDA uint8 tensor")
+            self._in = stream
+        else:
+            self._in = torch.from_numpy(np.frombuffer(stream, dtype=np.uint8).copy()).to(self._dev)
+        self._n, self._flags = self._in.numel(), 1 if fragment else 0
+        self._cuda = torch.cuda.current_stream(self._dev).cuda_stream
+        # the chunk table: encoder chunks hold 64 KiB each, and a data chunk is at least 8 bytes whatever wrote it
+        self._max_chunks = min(self._n // 1024 + 16, MAX_BATCH_CHUNKS)
+        self._index()
+        res = self._call([])[2]
+        if res.status.code == 202 and res.status.b == 1:
+            self._max_chunks = min(self._n // 8 + 16, MAX_BATCH_CHUNKS)
+            self._index()
+            res = self._call([])[2]
+        self._result = res
+        self.total = int(res.bytes)
+
+    def _index(self):
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        self._offs = torch.empty(self._max_chunks + 1, dtype=torch.int64, device=self._dev)
+        count = torch.empty(1, dtype=torch.int32, device=self._dev)
+        need = L.sb_frame_index_scratch_bytes(self._n, self._max_chunks)
+        scr = torch.empty(need, dtype=torch.uint8, device=self._dev)
+        e = _lib.SbError()
+        if L.sb_frame_index_device_ws(self._in.data_ptr(), self._n, self._flags, self._offs.data_ptr(), self._max_chunks,
+                                      count.data_ptr(), scr.data_ptr(), need, self._cuda, C.byref(e)):
+            raise from_c(e)
+        c = int(count.cpu().numpy().view(np.uint32)[0])
+        self._nchunks = None if c == 0xFFFFFFFF else c        # SB_FRAME_NOT_INDEXABLE: walked
+
+    def _call(self, ranges):
+        """One sb_frame_decode_ranges_device_ws call: (out_lens, statuses, stream result, output tensor, offsets)."""
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        k = len(ranges)
+        # a buffer needs only what the stream can give the range: nothing is written past min(lo + n, total)
+        total = getattr(self, "total", 0)
+        room = [max(0, min(n, total - lo)) for lo, n in ranges]
+        offs = np.zeros(k, dtype=np.int64)
+        if k:
+            offs[1:] = np.cumsum(room[:-1])
+        t_out = torch.empty(sum(room) + 1, dtype=torch.uint8, device=self._dev)
+        desc = np.array([lo for lo, _ in ranges] + [n for _, n in ranges], dtype=np.uint64).view(np.int64)
+        t_desc = torch.from_numpy(np.concatenate([desc, offs + t_out.data_ptr()])).to(self._dev)
+        t_res = torch.zeros(5 * k + 6, dtype=torch.int64, device=self._dev)   # out_lens, statuses, the stream result
+        need = L.sb_frame_decode_ranges_scratch_bytes(self._max_chunks, k)
+        scr = torch.empty(need, dtype=torch.uint8, device=self._dev)
+        e = _lib.SbError()
+        p = t_desc.data_ptr()
+        if L.sb_frame_decode_ranges_device_ws(self._in.data_ptr(), self._n,
+                                              self._offs.data_ptr() if self._nchunks is not None else None,
+                                              self._nchunks or 0, self._flags, p, p + 8 * k, p + 16 * k, t_res.data_ptr(),
+                                              t_res.data_ptr() + 8 * k, k, t_res.data_ptr() + 40 * k, scr.data_ptr(), need,
+                                              self._max_chunks, self._cuda, C.byref(e)):
+            raise from_c(e)
+        back = t_res.cpu().numpy().view(np.uint64)
+        res = _lib.SbFrameResult.from_buffer_copy(back[5 * k:].tobytes()[:C.sizeof(_lib.SbFrameResult)])
+        return back[:k], back[k:5 * k].reshape(k, 4), res, t_out, offs
+
+    def __len__(self):
+        return self.total
+
+    def read(self, lo: int, n: int) -> bytes:
+        """Decoded bytes [lo, lo + n), fewer at the end of the stream."""
+        return self.read_ranges([(lo, n)])[0]
+
+    def read_ranges(self, ranges) -> list:
+        """One bytes object per (lo, n) range. Ranges may be empty, unsorted, overlapping or repeated; each call to the
+        library takes a group of them whose staging and output stay bounded. Raises the first failing range's error."""
+        ranges = [(int(lo), int(n)) for lo, n in ranges]
+        for lo, n in ranges:
+            if lo < 0 or n < 0 or lo + n > 0xFFFFFFFFFFFFFFFF:
+                raise ValueError("range (%d, %d) is not within 64-bit offsets" % (lo, n))
+        out, i = [], 0
+        while i < len(ranges):
+            j, size = i, 0
+            while j < len(ranges) and j - i < self.RANGES_PER_CALL:
+                room = max(0, min(ranges[j][1], self.total - ranges[j][0]))
+                if j > i and size + room > self.BYTES_PER_CALL:
+                    break
+                size += room
+                j += 1
+            lens, sts, _, t_out, offs = self._call(ranges[i:j])
+            for s in sts:
+                if s[0] & 0xFFFFFFFF:
+                    raise from_c(_lib.SbError(int(s[0] & 0xFFFFFFFF), 0, int(s[1]), int(s[2]), int(s[3])))
+            back = t_out.cpu().numpy()
+            out += [back[o:o + int(m)].tobytes() for o, m in zip(offs, lens)]
+            i = j
+        return out
