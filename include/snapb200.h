@@ -321,6 +321,60 @@ int sb_frame_decode_ranges_device_ws(const uint8_t* d_in, uint64_t n, const uint
                                      uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, sb_frame_result* d_result,
                                      void* scratch, uint64_t scratch_bytes, uint32_t max_chunks, void* stream, sb_error* err);
 
+/* Seek table of one frame stream in device memory, built on the device once and then read by
+ * sb_frame_table_decode_ranges_device_ws any number of times without another pass over the stream's headers. The build
+ * runs sb_frame_decode_ranges_device_ws's index phase (d_chunk_offs/nchunks, flags bit0 and max_chunks, 1 .. 4,194,302,
+ * work as there) and writes the table to d_table, which must be 8-byte aligned and hold at least
+ * sb_frame_table_bytes(max_chunks) bytes. *d_result is what sb_frame_decode_ranges_device_ws writes with nranges == 0: the
+ * walk status, the decoded total and the chunk count.
+ *   The table is a header (a magic word with the format version, the stream's compressed length n, the chunk count, the
+ *   decoded total, the walk's stopping status, whether the chunk table was too small) and one 32-byte record per data
+ *   chunk in stream order (body offset and length, decoded length, expected CRC, type, decoded offset). It holds no
+ *   pointers, and its first sb_frame_table_bytes(result.nchunks) bytes are a complete table: it may be cut to that size,
+ *   copied or moved. A walked stream (padding or skippable chunks, a repeated identifier) is walked here, once; its table
+ *   lists only the data chunks.
+ * Scratch: sb_frame_table_build_scratch_bytes(max_chunks). Stream ordered, no allocation, no host synchronisation, a fixed
+ * number of launches. Null pointers, max_chunks out of range, nchunks > max_chunks with an index and a table or scratch
+ * that is too small are SB_E_INVALID with nothing launched. */
+uint64_t sb_frame_table_bytes(uint32_t nchunks);
+uint64_t sb_frame_table_build_scratch_bytes(uint32_t max_chunks);
+int sb_frame_table_build_device_ws(const uint8_t* d_in, uint64_t n, const uint64_t* d_chunk_offs, uint32_t nchunks,
+                                   uint32_t flags, void* d_table, uint64_t table_bytes, uint32_t max_chunks,
+                                   sb_frame_result* d_result, void* scratch, uint64_t scratch_bytes, void* stream,
+                                   sb_error* err);
+/* Byte ranges of many tabled frame streams in one call. d_tables, d_ins and d_in_lens are device arrays of `count`
+ * entries: stream u is d_ins[u][0 .. d_in_lens[u]) and d_tables[u] its seek table. Range r asks for decoded bytes
+ * [d_lo[r], d_lo[r] + d_len[r]) of stream d_unit[r] into d_out_ptrs[r] (device, d_len[r] bytes). Ranges may be empty,
+ * unsorted, overlapping, repeated, reach past the end and mix streams in any order; output buffers must not overlap each
+ * other or the inputs. Only the chunks a range covers are decoded and checksummed. With total the table's decoded total
+ * and end = min(lo + len, total), range r verifies chunk k (output offset off_k, decoded length dlen_k) iff
+ * off_k < end && off_k + max(dlen_k, 1) > lo. d_statuses[r] and d_out_lens[r], in priority order:
+ *   1. d_unit[r] >= count: SB_E_INVALID{a=unit, b=count, c=1}, 0;
+ *   2. d_tables[u] is not a table of this format, or was built over a stream of another length than d_in_lens[u]:
+ *      SB_E_INVALID{a=d_in_lens[u], b=the table's n (0 if it is not a table), c=2}, 0;
+ *   3. the chunk table of the build was too small: SB_E_INVALID{a=max_chunks, b=1}, 0;
+ *   4. a verified chunk fails: the first in stream order, k*, with its own status; max(off_k*, lo) - lo;
+ *   5. the range reaches past total and the build's header walk stopped on an error: that error; max(end - lo, 0);
+ *   6. otherwise Ok; max(end - lo, 0) (a range past a clean end is a short read, like pread).
+ *   For a table built from stream S, every range gets exactly the status, out_len and bytes that
+ *   sb_frame_decode_ranges_device_ws(S, ...) gives it with the same index, flags and max_chunks. Nothing outside
+ *   [out_r, out_r + max(end - lo, 0)) is written.
+ *   Tables are checked only as far as is cheap. Every decoded chunk is still CRC-checked, so a table paired with other
+ *   bytes of the same length gives errors, not wrong output. A record a range uses must keep to the bounds every build
+ *   writes (body inside the stream, body <= 76,490 bytes, decoded <= 65,536 bytes, a data chunk type, a non-negative
+ *   slice of [lo, end)), else it fails as chunk k with SB_E_INVALID{a=k, b=0, c=3}; no table content makes the call read
+ *   outside a stream or write outside a range's buffer or the scratch.
+ * A chunk shared by several ranges is decoded once per range; the scratch, sb_frame_table_ranges_scratch_bytes(nranges)
+ * bytes, holds 128 KiB of staging per range. Stream ordered, no allocation, no host synchronisation, and the same
+ * launches whatever count and nranges; nranges == 0 does nothing. Null pointers that are needed, count or
+ * nranges >= 2^31 and scratch that is too small are SB_E_INVALID with nothing launched. */
+uint64_t sb_frame_table_ranges_scratch_bytes(uint32_t nranges);
+int sb_frame_table_decode_ranges_device_ws(const void* const* d_tables, const uint8_t* const* d_ins,
+                                           const uint64_t* d_in_lens, uint32_t count, const uint32_t* d_unit,
+                                           const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                                           uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
+                                           uint64_t scratch_bytes, void* stream, sb_error* err);
+
 /* Chunk index of a frame stream in device memory, built in parallel on the device:
  * the offset of every chunk header in d_in[0..n) followed by n -- exactly the
  * d_chunk_offs that sb_frame_decode_device_ws accepts (max_chunks + 1 entries).

@@ -25,6 +25,7 @@
 #include "k10_frame_batch_encode.cuh"
 #include "k11_frame_batch_decode.cuh"
 #include "k12_frame_range_decode.cuh"
+#include "k13_frame_table.cuh"
 
 namespace {
 
@@ -111,6 +112,12 @@ __global__ void __launch_bounds__(1024) k12_plan_tiles_kernel(sbk::RangePlan q) 
 // with the occupancy hint ptxas keeps the pair lookup in registers across K5's decode (without it: 64 and a 4-byte spill)
 __global__ void __launch_bounds__(128, 4) k12_decode_kernel(sbk::RangePlan q) { sbk::k12_decode_body(q); }
 __global__ void __launch_bounds__(256) k12_finish_kernel(sbk::RangePlan q) { sbk::k12_finish_body(q); }
+__global__ void __launch_bounds__(256) k13_export_kernel(sbk::DecodePlan p, sbk::TableHead* t) { sbk::k13_export_body(p, t); }
+__global__ void __launch_bounds__(1024) k13_plan_kernel(sbk::TablePlan q) { sbk::k13_plan_body(q); }
+__global__ void __launch_bounds__(1024) k13_plan_tiles_kernel(sbk::TablePlan q) { sbk::k13_plan_tiles_body(q); }
+// K12's decode budget: 4 CTAs of 128 per SM at least
+__global__ void __launch_bounds__(128, 4) k13_decode_kernel(sbk::TablePlan q) { sbk::k13_decode_body(q); }
+__global__ void __launch_bounds__(128) k13_finish_kernel(sbk::TablePlan q) { sbk::k13_finish_body(q); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -716,6 +723,33 @@ int launch_frame_range_decode(Ctx& c, const uint8_t* d_in, uint64_t n, const uin
     return 0;
 }
 
+// ---- seek tables (K5's index phase, then K13's export) and ranges over tabled streams (K13)
+int launch_frame_table_build(Ctx& c, const uint8_t* d_in, uint64_t n, const uint64_t* d_chunk_offs, uint32_t nchunks,
+                             uint32_t flags, void* d_table, uint32_t max_chunks, sb_frame_result* d_result, void* scratch,
+                             cudaStream_t st, sb_error* err) {
+    const sbk::DecodePlan p = make_decode_plan(d_in, n, nullptr, ~0ull, d_chunk_offs, nchunks, (int)(flags & 1u), d_result,
+                                               scratch, max_chunks);
+    int rc = decode_index_phase(c, p, st, err);
+    if (rc) return rc;
+    k13_export_kernel<<<(unsigned)(((uint64_t)max_chunks + 1 + 255) / 256), 256, 0, st>>>(p, (sbk::TableHead*)d_table);
+    g_launches++;
+    CK(cudaGetLastError());
+    return 0;
+}
+int launch_frame_table_ranges(Ctx& c, const sbk::TablePlan& q, cudaStream_t st, sb_error* err) {
+    // the pair total is on the device: 4 warps per CTA, at most 16 CTAs per SM, grid-stride beyond that
+    const uint64_t most = (uint64_t)16 * c.sms, fw = ((uint64_t)q.nranges + 3) / 4;
+    const unsigned ptiles = (unsigned)(((uint64_t)q.nranges + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    const uint32_t smem = sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP;
+    k13_plan_kernel<<<ptiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k13_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    k13_decode_kernel<<<(unsigned)most, 128, smem + 4 * sizeof(sb_error), st>>>(q);
+    k13_finish_kernel<<<fw < most ? (unsigned)fw : (unsigned)most, 128, smem, st>>>(q);
+    g_launches += 4;
+    CK(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace
 
 // =========================================================================
@@ -922,6 +956,56 @@ int sb_frame_decode_ranges_device_ws(const uint8_t* d_in, uint64_t n, const uint
     if (rc) return rc;
     rc = launch_frame_range_decode(*c, d_in, n, d_chunk_offs, nchunks, flags, d_lo, d_len, d_out_ptrs, d_out_lens, d_statuses,
                                    nranges, d_result, scratch, max_chunks, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_frame_table_bytes(uint32_t nchunks) { return sbk::k13_table_bytes(nchunks); }
+uint64_t sb_frame_table_build_scratch_bytes(uint32_t max_chunks) { return decode_ws_bytes(max_chunks); }
+
+int sb_frame_table_build_device_ws(const uint8_t* d_in, uint64_t n, const uint64_t* d_chunk_offs, uint32_t nchunks,
+                                   uint32_t flags, void* d_table, uint64_t table_bytes, uint32_t max_chunks,
+                                   sb_frame_result* d_result, void* scratch, uint64_t scratch_bytes, void* stream,
+                                   sb_error* err) {
+    if ((!d_in && n) || !d_table || !d_result || !scratch) return fail(err, SB_E_INVALID);
+    if (max_chunks == 0 || max_chunks > sbk::K12_MAX_CHUNKS) return fail(err, SB_E_INVALID, max_chunks, sbk::K12_MAX_CHUNKS);
+    if (d_chunk_offs && nchunks > max_chunks) return fail(err, SB_E_INVALID, nchunks, max_chunks);
+    if (table_bytes < sbk::k13_table_bytes(max_chunks)) return fail(err, SB_E_INVALID, table_bytes, sbk::k13_table_bytes(max_chunks));
+    if (scratch_bytes < decode_ws_bytes(max_chunks)) return fail(err, SB_E_INVALID, scratch_bytes, decode_ws_bytes(max_chunks));
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_frame_table_build(*c, d_in, n, d_chunk_offs, nchunks, flags, d_table, max_chunks, d_result, scratch,
+                                  (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_frame_table_ranges_scratch_bytes(uint32_t nranges) { return sbk::k13_carve(nullptr, nranges, nullptr); }
+
+int sb_frame_table_decode_ranges_device_ws(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens,
+                                           uint32_t count, const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len,
+                                           uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
+                                           uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream,
+                                           sb_error* err) {
+    if (count >= sbk::K13_MAX_COUNT) return fail(err, SB_E_INVALID, count, sbk::K13_MAX_COUNT);
+    if (nranges >= sbk::K12_MAX_RANGES) return fail(err, SB_E_INVALID, nranges, sbk::K12_MAX_RANGES);
+    if (nranges == 0) { ok(err); return 0; }
+    if (count && (!d_tables || !d_ins || !d_in_lens)) return fail(err, SB_E_INVALID);
+    if (!d_unit || !d_lo || !d_len || !d_out_ptrs || !d_out_lens || !d_statuses || !scratch) return fail(err, SB_E_INVALID);
+    const uint64_t need = sbk::k13_carve(nullptr, nranges, nullptr);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    sbk::TablePlan q;
+    memset(&q, 0, sizeof q);
+    q.tables = d_tables; q.ins = d_ins; q.in_lens = d_in_lens; q.count = count;
+    q.unit = d_unit; q.lo = d_lo; q.len = d_len; q.outs = d_out_ptrs; q.out_lens = d_out_lens; q.statuses = d_statuses;
+    sbk::k13_carve(scratch, nranges, &q);
+    rc = launch_frame_table_ranges(*c, q, (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;

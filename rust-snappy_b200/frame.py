@@ -287,3 +287,136 @@ class RangeReader:
             out += [back[o:o + int(m)].tobytes() for o, m in zip(offs, lens)]
             i = j
         return out
+
+
+class TableReader:
+    """Random access to the decoded bytes of many frame streams on the device. Each stream gets a seek table, built once
+    on the device: a pointer-free list of its data chunks with their decoded offsets. `read_ranges([(i, lo, n), ...])`
+    then serves ranges of any of the streams in one library call per group, decoding and checksumming only the chunks
+    they cover, with no pass over any stream's headers. Every range gives what `RangeReader(streams[i]).read(lo, n)`
+    gives. A stream is a bytes-like object (uploaded once) or a contiguous 1-D CUDA uint8 tensor (kept alive).
+    fragment: the streams have no identifier. Calls run on the current torch stream and wait for their results."""
+
+    RANGES_PER_CALL = RangeReader.RANGES_PER_CALL
+    BYTES_PER_CALL = RangeReader.BYTES_PER_CALL
+
+    def __init__(self, streams, fragment=False):
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        self._dev = torch.device("cuda", torch.cuda.current_device())
+        self._cuda = torch.cuda.current_stream(self._dev).cuda_stream
+        self._ins = []
+        for s in streams:
+            if isinstance(s, torch.Tensor):
+                if not s.is_cuda or s.dtype != torch.uint8 or s.dim() != 1 or not s.is_contiguous():
+                    raise ValueError("TableReader takes contiguous 1-D CUDA uint8 tensors")
+                self._ins.append(s)
+            else:
+                self._ins.append(torch.from_numpy(np.frombuffer(s, dtype=np.uint8).copy()).to(self._dev))
+        flags = 1 if fragment else 0
+        count = len(self._ins)
+        # the chunk table as RangeReader sizes it: encoder chunks hold 64 KiB, and any data chunk is at least 8 bytes
+        caps = [min(t.numel() // 1024 + 16, MAX_BATCH_CHUNKS) for t in self._ins]
+        tables, results = self._build(range(count), caps, flags)
+        redo = [i for i in range(count) if results[i].status.code == 202 and results[i].status.b == 1]
+        if redo:
+            for i in redo:
+                caps[i] = min(self._ins[i].numel() // 8 + 16, MAX_BATCH_CHUNKS)
+            more, res2 = self._build(redo, [caps[i] for i in redo], flags)
+            for j, i in enumerate(redo):
+                tables[i], results[i] = more[j], res2[j]
+        # keep each table at its exact size
+        self._tables = [t[:L.sb_frame_table_bytes(r.nchunks)].clone() for t, r in zip(tables, results)]
+        self.lengths = [int(r.bytes) for r in results]
+        to64 = lambda v: torch.from_numpy(np.array(v, dtype=np.uint64).view(np.int64)).to(self._dev)
+        self._t_tables = to64([t.data_ptr() for t in self._tables] + [0])
+        self._t_ins = to64([t.data_ptr() for t in self._ins] + [0])
+        self._t_lens = to64([t.numel() for t in self._ins] + [0])
+
+    def _build(self, which, caps, flags):
+        """One sb_frame_table_build_device_ws per stream, one wait for all: (tables, results)."""
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        which = list(which)
+        need = max([L.sb_frame_table_build_scratch_bytes(c) for c in caps] + [1])
+        scr = torch.empty(need, dtype=torch.uint8, device=self._dev)
+        rsz = C.sizeof(_lib.SbFrameResult)
+        t_res = torch.zeros(max(len(which), 1) * rsz, dtype=torch.uint8, device=self._dev)
+        tables = []
+        for j, (i, cap) in enumerate(zip(which, caps)):
+            t_in = self._ins[i]
+            tb = L.sb_frame_table_bytes(cap)
+            table = torch.empty(tb, dtype=torch.uint8, device=self._dev)
+            e = _lib.SbError()
+            if L.sb_frame_table_build_device_ws(t_in.data_ptr(), t_in.numel(), None, 0, flags, table.data_ptr(), tb, cap,
+                                                t_res.data_ptr() + j * rsz, scr.data_ptr(), need, self._cuda, C.byref(e)):
+                raise from_c(e)
+            tables.append(table)
+        back = t_res.cpu().numpy().tobytes()
+        return tables, [_lib.SbFrameResult.from_buffer_copy(back[j * rsz:(j + 1) * rsz]) for j in range(len(which))]
+
+    def __len__(self):
+        return len(self._ins)
+
+    def _call(self, ranges):
+        """One sb_frame_table_decode_ranges_device_ws call: (out_lens, statuses, output tensor, offsets)."""
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        k = len(ranges)
+        room = [max(0, min(n, self.lengths[i] - lo)) for i, lo, n in ranges]
+        offs = np.zeros(k, dtype=np.int64)
+        if k:
+            offs[1:] = np.cumsum(room[:-1])
+        t_out = torch.empty(sum(room) + 1, dtype=torch.uint8, device=self._dev)
+        desc = np.array([lo for _, lo, _ in ranges] + [n for _, _, n in ranges], dtype=np.uint64).view(np.int64)
+        units = np.array([i for i, _, _ in ranges] + [0], dtype=np.uint32).view(np.int32)
+        t_desc = torch.from_numpy(np.concatenate([desc, offs + t_out.data_ptr()])).to(self._dev)
+        t_unit = torch.from_numpy(units).to(self._dev)
+        t_res = torch.zeros(5 * k, dtype=torch.int64, device=self._dev)       # out_lens, statuses
+        need = L.sb_frame_table_ranges_scratch_bytes(k)
+        scr = torch.empty(need, dtype=torch.uint8, device=self._dev)
+        e = _lib.SbError()
+        p = t_desc.data_ptr()
+        if L.sb_frame_table_decode_ranges_device_ws(self._t_tables.data_ptr(), self._t_ins.data_ptr(),
+                                                    self._t_lens.data_ptr(), len(self._ins), t_unit.data_ptr(), p,
+                                                    p + 8 * k, p + 16 * k, t_res.data_ptr(), t_res.data_ptr() + 8 * k, k,
+                                                    scr.data_ptr(), need, self._cuda, C.byref(e)):
+            raise from_c(e)
+        back = t_res.cpu().numpy().view(np.uint64)
+        return back[:k], back[k:5 * k].reshape(k, 4), t_out, offs
+
+    def read(self, i: int, lo: int, n: int) -> bytes:
+        """Decoded bytes [lo, lo + n) of stream i, fewer at the end of the stream."""
+        return self.read_ranges([(i, lo, n)])[0]
+
+    def read_ranges(self, ranges) -> list:
+        """One bytes object per (i, lo, n) range of stream i. Ranges may mix streams in any order and be empty,
+        unsorted, overlapping or repeated; each library call takes a group of them whose staging and output stay
+        bounded. Raises the first failing range's error."""
+        ranges = [(int(i), int(lo), int(n)) for i, lo, n in ranges]
+        for i, lo, n in ranges:
+            if not 0 <= i < len(self._ins):
+                raise IndexError("stream %d of %d" % (i, len(self._ins)))
+            if lo < 0 or n < 0 or lo + n > 0xFFFFFFFFFFFFFFFF:
+                raise ValueError("range (%d, %d) is not within 64-bit offsets" % (lo, n))
+        out, a = [], 0
+        while a < len(ranges):
+            b, size = a, 0
+            while b < len(ranges) and b - a < self.RANGES_PER_CALL:
+                i, lo, n = ranges[b]
+                room = max(0, min(n, self.lengths[i] - lo))
+                if b > a and size + room > self.BYTES_PER_CALL:
+                    break
+                size += room
+                b += 1
+            lens, sts, t_out, offs = self._call(ranges[a:b])
+            for s in sts:
+                if s[0] & 0xFFFFFFFF:
+                    raise from_c(_lib.SbError(int(s[0] & 0xFFFFFFFF), 0, int(s[1]), int(s[2]), int(s[3])))
+            back = t_out.cpu().numpy()
+            out += [back[o:o + int(m)].tobytes() for o, m in zip(offs, lens)]
+            a = b
+        return out
