@@ -60,14 +60,15 @@ __device__ unsigned long long g_k1_prof[18];
 #define K1_PROF_FLUSH do { } while (0)
 #if defined(SB_EMU)
 // CPU warp-emulator build (tests/emu): the same window counts, readable by the tests through the symbol
-extern "C" { __attribute__((weak)) unsigned long long sb_emu_k1_windows[3]; }
+extern "C" { __attribute__((weak)) unsigned long long sb_emu_k1_windows[4]; }
 #define K1_COUNT(k) do { if (sbk::lane_id() == 0) sb_emu_k1_windows[k]++; } while (0)
 #else
 #define K1_COUNT(k) do { } while (0)
 #endif
 #endif
 // K1_COUNT: [0] fast-path windows whose probe the previous window issued (hoisted), [1] probes issued at the loop top;
-// emulator build only: [2] probes whose table slot changed between the read and the use (must stay 0)
+// emulator build only: [2] probes whose table slot changed between the read and the use, [3] sequential-word fetches
+// that reach byte n of the block (both must stay 0)
 
 namespace sbk {
 
@@ -261,9 +262,14 @@ struct K1Pre {
 // the four sequential words a lane needs for a window, fetched one window ahead when the
 // window lives in global memory (hides one L2 round trip per window)
 struct K1Seq { uint32_t a0, a1, a2, a3, a4, w; };
-SB_DEVICE K1Seq k1_fetch_seq(const uint8_t* win, uint32_t w) {
+SB_DEVICE K1Seq k1_fetch_seq(const uint8_t* win, uint32_t w, uint32_t n) {
     const uintptr_t aa = (uintptr_t)(win + w + lane_id());
     const uint32_t* aw = (const uint32_t*)(aa & ~(uintptr_t)3);
+#ifdef SB_EMU
+    if (any((const uint8_t*)(aw + 5) > win + n)) K1_COUNT(3);   // a word reaches byte n or beyond (must stay 0)
+#else
+    (void)n;
+#endif
     K1Seq q;
     q.a0 = aw[0]; q.a1 = aw[1]; q.a2 = aw[2]; q.a3 = aw[3]; q.a4 = aw[4]; q.w = w;
     return q;
@@ -428,6 +434,10 @@ SB_DEVICE bool k1_finish(const uint8_t* win, uint32_t n, uint16_t* table, unsign
     // ---- exit state and copy-end insert
     // (warp-uniform values, written as selects: only the copy-end insert below is a branch)
     const uint32_t ncopy = popc(CS);
+    // hash of the word at e - 1 for a copy ending at e in 33..64 (the copy-end insert below), fetched by every lane for
+    // its own copy end while the reduction that finds the last copy runs, instead of by index after it
+    const unsigned nsh = (unsigned)((uintptr_t)(win + nxt->w + lane) & 3u) * 8;
+    const uint32_t hend = shfl(K1_HASH(funnel_r(nxt->a0, nxt->a1, nsh)), (lane + L - 33) & 31u);
     const uint32_t e_last = reduce_max(taken ? lane + L : 0u);    // end of the window's last copy, 0 without one
     const bool over = e_last >= 32;                               // that copy ends at or beyond the window's end
     // else the window ends in a scan: probes since the last copy end, since the rematch miss at i0, or the running scan's
@@ -440,10 +450,8 @@ SB_DEVICE bool k1_finish(const uint8_t* win, uint32_t n, uint16_t* table, unsign
             // ... but inside the next one, whose sequential words are already prefetched: take
             // its hash from the lane that holds it instead of paying a global load (:293-295)
             if (st.s < s_limit) {
-                const unsigned nsh = (unsigned)((uintptr_t)(win + nxt->w + lane) & 3u) * 8;
-                const uint32_t hsel = shfl(K1_HASH(funnel_r(nxt->a0, nxt->a1, nsh)), e_last - 33);
                 syncwarp();
-                if (lane == 0) table[hsel] = (uint16_t)(st.s - 1);
+                if (taken && lane + L == e_last) table[hend] = (uint16_t)(st.s - 1);   // the last copy's lane
                 syncwarp();
             }
         } else {
@@ -495,9 +503,9 @@ SB_DEVICE void k1_parse(const uint8_t* win, uint32_t n, uint16_t* table, const K
             bool ok = false;
             if (fast) {
                 K1Seq nxt = seq;
-                if (w + 100 < n) nxt = k1_fetch_seq(win, w + 32);   // issue next window's loads now
+                if (w + 100 < n) nxt = k1_fetch_seq(win, w + 32, n);   // issue next window's loads now
                 K1_TICK(0);                                          // [0] loop top / state checks / prefetch issue
-                K1Seq cur = seq.w == w ? seq : k1_fetch_seq(win, w);
+                K1Seq cur = seq.w == w ? seq : k1_fetch_seq(win, w, n);
                 K1Probe pb = k1_probe_issue(win, table, shift, cur);
                 K1_COUNT(1);
                 // While a window issues its successor's probe (`hoisted`), the successor runs in this inner loop
@@ -526,7 +534,10 @@ SB_DEVICE void k1_parse(const uint8_t* win, uint32_t n, uint16_t* table, const K
                     K1_TICK(1);
                     // unconditional (the current window when w + 32 is too close to the end): a conditional load
                     // would become register moves that wait for it
-                    nxt = k1_fetch_seq(win, w + 100 < n ? w + 32 : w);
+                    nxt = k1_fetch_seq(win, w + 100 < n ? w + 32 : w, n);
+                    // the words four windows ahead come from HBM: have L2 fetch them now, so that the load above
+                    // finds them in L2 when its turn comes (a prefetch has no register to wait for)
+                    prefetch_l2(win + (w + 128 + lane < n ? w + 128 + lane : n - 1));
                 }
             }
             if (!ok) { K1_TICK(8); finished = k1_serial(win, n, table, shift, s_limit, st, w + 32, ring, prod); K1_TICK(9); }   // [9] serial path

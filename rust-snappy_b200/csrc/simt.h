@@ -14,6 +14,10 @@
 #ifndef SB_EMU_PRIMITIVES
 #error "SB_EMU builds must include tests/emu/simt_emu.h first (it defines the warp primitives)"
 #endif
+namespace sbk {
+// the emulator has no caches: a prefetch is a hint with nothing to do
+SB_DEVICE void prefetch_l2(const void*) {}
+}
 #else
 
 #include <cuda_runtime.h>
@@ -76,6 +80,8 @@ SB_DEVICE void spin_long() { __nanosleep(1500); }
 SB_DEVICE uint32_t ld_volatile(const uint32_t* p) { return *(const volatile uint32_t*)p; }
 SB_DEVICE void st_volatile(uint32_t* p, uint32_t v) { *(volatile uint32_t*)p = v; }
 SB_DEVICE uint64_t ld_volatile64(const uint64_t* p) { return *(const volatile uint64_t*)p; }
+// L2 prefetch: no destination register, so nothing waits for it
+SB_DEVICE void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
 
 // read-only / streaming global accessors
 SB_DEVICE uint32_t ldg32(const void* p) { return __ldg((const uint32_t*)p); }
