@@ -342,6 +342,36 @@ int sb_frame_table_build_device_ws(const uint8_t* d_in, uint64_t n, const uint64
                                    uint32_t flags, void* d_table, uint64_t table_bytes, uint32_t max_chunks,
                                    sb_frame_result* d_result, void* scratch, uint64_t scratch_bytes, void* stream,
                                    sb_error* err);
+/* Seek tables of a batch of frame streams in one call, every unit indexed in parallel: what one
+ * sb_frame_table_build_device_ws per stream gives, without a call per stream. Unit i is batch input i (in_ptrs or
+ * in_base + stride, in_lens or the uniform length, count); the out_* fields, out_lens and statuses are not read. flags
+ * bit0, d_chunk_offs/d_index_at (both or neither), in_bytes and max_chunks (1 .. 4,194,302) mean exactly what they mean
+ * for sb_frame_decode_batch_device_ws: units take ranges of one chunk table of max_chunks slots in batch order, an index
+ * that does not describe its unit costs speed, never a result, and lengths summing past in_bytes get units walked with
+ * exact results.
+ *   The tables are packed back to back in batch order into d_tables (device, 8-byte aligned, at least
+ *   sb_frame_table_batch_bytes(count, max_chunks) = 64 * count + 32 * max_chunks bytes). d_table_offs (device, count + 1
+ *   entries) gets d_table_offs[0] = 0 and d_table_offs[i + 1] = d_table_offs[i] + sb_frame_table_bytes(d_results[i].nchunks):
+ *   every table size is a multiple of 32, so every table is 8-byte aligned, and the first d_table_offs[count] bytes may be
+ *   kept with one copy.
+ *   A unit that fits the chunk table gets a table and d_results[i] byte-identical (padding included) to the first
+ *   sb_frame_table_bytes(nchunks) bytes of what sb_frame_table_build_device_ws writes for that stream alone with the same
+ *   flags, its own index slice or none, and a max_chunks large enough: walked streams, fragments, corrupt chunks (a build
+ *   checks no CRC), truncated streams and decoded totals over 2^32 alike. The first unit that does not fit and every unit
+ *   after it get d_results[i] = {SB_E_INVALID{a=max_chunks, b=1}, 0, 0} and a 64-byte table (the stream's length, total 0,
+ *   no chunks, chunk table too small, that status): every read of it gives that status and no bytes.
+ * Scratch: sb_frame_table_build_batch_scratch_bytes(count, in_bytes, max_chunks), need not be zeroed. Stream ordered, no
+ * allocation, no host synchronisation, and the same launches whatever count and the streams hold (one number with an
+ * index, one without). Null pointers (batch, d_tables, d_table_offs, d_results, scratch), count >= 2^31, max_chunks out of
+ * range, an index given half and tables or scratch that are too small are SB_E_INVALID with nothing launched; count == 0
+ * does nothing. */
+uint64_t sb_frame_table_batch_bytes(uint32_t count, uint32_t max_chunks);
+uint64_t sb_frame_table_build_batch_scratch_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks);
+int sb_frame_table_build_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t flags,
+                                         const uint64_t* d_chunk_offs, const uint64_t* d_index_at, uint32_t max_chunks,
+                                         void* d_tables, uint64_t tables_bytes, uint64_t* d_table_offs,
+                                         sb_frame_result* d_results, void* scratch, uint64_t scratch_bytes, void* stream,
+                                         sb_error* err);
 /* Byte ranges of many tabled frame streams in one call. d_tables, d_ins and d_in_lens are device arrays of `count`
  * entries: stream u is d_ins[u][0 .. d_in_lens[u]) and d_tables[u] its seek table. Range r asks for decoded bytes
  * [d_lo[r], d_lo[r] + d_len[r]) of stream d_unit[r] into d_out_ptrs[r] (device, d_len[r] bytes). Ranges may be empty,

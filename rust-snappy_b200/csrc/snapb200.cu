@@ -26,6 +26,7 @@
 #include "k11_frame_batch_decode.cuh"
 #include "k12_frame_range_decode.cuh"
 #include "k13_frame_table.cuh"
+#include "k14_frame_table_batch.cuh"
 
 namespace {
 
@@ -118,6 +119,9 @@ __global__ void __launch_bounds__(1024) k13_plan_tiles_kernel(sbk::TablePlan q) 
 // K12's decode budget: 4 CTAs of 128 per SM at least
 __global__ void __launch_bounds__(128, 4) k13_decode_kernel(sbk::TablePlan q) { sbk::k13_decode_body(q); }
 __global__ void __launch_bounds__(128) k13_finish_kernel(sbk::TablePlan q) { sbk::k13_finish_body(q); }
+__global__ void __launch_bounds__(1024) k14_size_local_kernel(sbk::TableBatchPlan t) { sbk::k14_size_local_body(t); }
+__global__ void __launch_bounds__(1024) k14_size_tiles_kernel(sbk::TableBatchPlan t) { sbk::k14_size_tiles_body(t); }
+__global__ void __launch_bounds__(256) k14_export_kernel(sbk::TableBatchPlan t) { sbk::k14_export_body(t); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -648,48 +652,89 @@ int launch_frame_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint64_t* d
 uint64_t frame_decode_batch_ws_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks) {
     return sbk::k11_carve(nullptr, count, in_bytes, max_chunks, nullptr);
 }
-int launch_frame_decode_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t flags, const uint64_t* d_chunk_offs,
-                              const uint64_t* d_index_at, uint32_t max_chunks, uint32_t* d_unit_chunks, void* scratch,
-                              cudaStream_t st, sb_error* err) {
+// grids over lists whose true lengths are on the device: at most `per_sm` CTAs per SM, grid-stride beyond that
+unsigned device_grid(const Ctx& c, uint64_t items, unsigned per_cta, unsigned per_sm) {
+    const uint64_t g = (items + per_cta - 1) / per_cta, most = (uint64_t)per_sm * c.sms;
+    return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most;
+}
+sbk::FrameDecodeBatchPlan make_frame_decode_batch_plan(const sb_batch& b, uint64_t in_bytes, uint32_t flags,
+                                                       const uint64_t* d_chunk_offs, const uint64_t* d_index_at,
+                                                       uint32_t max_chunks, uint32_t* d_unit_chunks, void* scratch) {
     sbk::FrameDecodeBatchPlan q;
     memset(&q, 0, sizeof q);
     q.b = b; q.fragment = flags & 1u; q.cidx = d_chunk_offs; q.cidx_at = d_index_at; q.unit_chunks = d_unit_chunks;
     const uint64_t want = k7_want_seg();
     q.seg = want < sbk::K7_SEG_MIN ? sbk::K7_SEG_MIN : want > (1ull << 31) ? (1ull << 31) : want;
     sbk::k11_carve(scratch, b.count, in_bytes, max_chunks, &q);
-    // grids over lists whose true lengths are on the device: at most `per_sm` CTAs per SM, grid-stride beyond that
-    auto grid = [&](uint64_t items, unsigned per_cta, unsigned per_sm) {
-        const uint64_t g = (items + per_cta - 1) / per_cta, most = (uint64_t)per_sm * c.sms;
-        return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most;
-    };
-    const unsigned utiles = (unsigned)(((uint64_t)b.count + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    return q;
+}
+// K11's index part, k11_plan .. k11_oscan_tiles: afterwards the scratch holds every fitting unit's chunk records, live
+// count, walk status and decoded offsets. Nothing here reads the out_* fields.
+int frame_decode_batch_index(Ctx& c, const sbk::FrameDecodeBatchPlan& q, cudaStream_t st, sb_error* err) {
+    const uint32_t count = q.b.count, max_chunks = q.max_chunks;
+    const unsigned utiles = (unsigned)(((uint64_t)count + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
     const unsigned stiles = (unsigned)(((uint64_t)max_chunks + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
     CK(cudaMemsetAsync(q.in_total, 0, sizeof *q.in_total, st));
     k11_plan_kernel<<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
     k11_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
-    if (d_chunk_offs) {
-        k11_link_kernel<<<grid((uint64_t)max_chunks + b.count, 256, 16), 256, 0, st>>>(q);
+    if (q.cidx) {
+        k11_link_kernel<<<device_grid(c, (uint64_t)max_chunks + count, 256, 16), 256, 0, st>>>(q);
         g_launches += 3;
     } else {
-        k11_survivors_kernel<<<grid(q.nseg_cap, 4, 16), 128, 0, st>>>(q);
-        k11_stitch_kernel<<<b.count < (uint32_t)(8 * c.sms) ? b.count : (unsigned)(8 * c.sms), sbk::K7_STITCH_THREADS,
+        k11_survivors_kernel<<<device_grid(c, q.nseg_cap, 4, 16), 128, 0, st>>>(q);
+        k11_stitch_kernel<<<count < (uint32_t)(8 * c.sms) ? count : (unsigned)(8 * c.sms), sbk::K7_STITCH_THREADS,
                             sbk::K7_STITCH_SMEM, st>>>(q);
         g_launches += 4;
     }
     k11_count_kernel<<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
     k11_range_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
     g_launches += 2;
-    if (!d_chunk_offs) {
-        k11_emit_kernel<<<grid(q.nseg_cap, 128, 16), 128, 0, st>>>(q);
+    if (!q.cidx) {
+        k11_emit_kernel<<<device_grid(c, q.nseg_cap, 128, 16), 128, 0, st>>>(q);
         g_launches++;
     }
-    k11_parse_kernel<<<grid(max_chunks, 256, 16), 256, 0, st>>>(q);
-    k11_fill_kernel<<<grid(b.count, 64, 32), 64, 0, st>>>(q);
+    k11_parse_kernel<<<device_grid(c, max_chunks, 256, 16), 256, 0, st>>>(q);
+    k11_fill_kernel<<<device_grid(c, count, 64, 32), 64, 0, st>>>(q);
     k11_oscan_local_kernel<<<stiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
     k11_oscan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
-    k11_decode_kernel<<<grid(max_chunks, 4, 16), 128, sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
-    k11_finish_kernel<<<grid(b.count, 256, 16), 256, 0, st>>>(q);
-    g_launches += 6;
+    g_launches += 4;
+    CK(cudaGetLastError());
+    return 0;
+}
+int launch_frame_decode_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t flags, const uint64_t* d_chunk_offs,
+                              const uint64_t* d_index_at, uint32_t max_chunks, uint32_t* d_unit_chunks, void* scratch,
+                              cudaStream_t st, sb_error* err) {
+    const sbk::FrameDecodeBatchPlan q = make_frame_decode_batch_plan(b, in_bytes, flags, d_chunk_offs, d_index_at, max_chunks,
+                                                                     d_unit_chunks, scratch);
+    int rc = frame_decode_batch_index(c, q, st, err);
+    if (rc) return rc;
+    // the payload part: decode + CRC, then the results
+    k11_decode_kernel<<<device_grid(c, max_chunks, 4, 16), 128, sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    k11_finish_kernel<<<device_grid(c, b.count, 256, 16), 256, 0, st>>>(q);
+    g_launches += 2;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// ---- seek tables of a batch (K11's index part, then K14's size scan and export)
+uint64_t table_batch_ws_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks) {
+    return sbk::k14_carve(nullptr, count, in_bytes, max_chunks, nullptr);
+}
+int launch_frame_table_build_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t flags, const uint64_t* d_chunk_offs,
+                                   const uint64_t* d_index_at, uint32_t max_chunks, void* d_tables, uint64_t* d_table_offs,
+                                   sb_frame_result* d_results, void* scratch, cudaStream_t st, sb_error* err) {
+    sbk::TableBatchPlan t;
+    memset(&t, 0, sizeof t);
+    t.q = make_frame_decode_batch_plan(b, in_bytes, flags, d_chunk_offs, d_index_at, max_chunks, nullptr, scratch);
+    sbk::k14_carve(scratch, b.count, in_bytes, max_chunks, &t);
+    t.tables = (uint8_t*)d_tables; t.table_offs = d_table_offs; t.results = d_results;
+    int rc = frame_decode_batch_index(c, t.q, st, err);
+    if (rc) return rc;
+    const unsigned utiles = (unsigned)(((uint64_t)b.count + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    k14_size_local_kernel<<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(t);
+    k14_size_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(t);
+    k14_export_kernel<<<device_grid(c, (uint64_t)max_chunks + b.count + 1, 256, 16), 256, 0, st>>>(t);
+    g_launches += 3;
     CK(cudaGetLastError());
     return 0;
 }
@@ -978,6 +1023,34 @@ int sb_frame_table_build_device_ws(const uint8_t* d_in, uint64_t n, const uint64
     if (rc) return rc;
     rc = launch_frame_table_build(*c, d_in, n, d_chunk_offs, nchunks, flags, d_table, max_chunks, d_result, scratch,
                                   (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_frame_table_batch_bytes(uint32_t count, uint32_t max_chunks) { return sbk::k14_tables_bytes(count, max_chunks); }
+uint64_t sb_frame_table_build_batch_scratch_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks) {
+    return table_batch_ws_bytes(count, in_bytes, max_chunks);
+}
+
+int sb_frame_table_build_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t flags, const uint64_t* d_chunk_offs,
+                                         const uint64_t* d_index_at, uint32_t max_chunks, void* d_tables,
+                                         uint64_t tables_bytes, uint64_t* d_table_offs, sb_frame_result* d_results,
+                                         void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if (!batch || !d_tables || !d_table_offs || !d_results || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K11_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K11_MAX_COUNT);
+    if (!d_chunk_offs != !d_index_at) return fail(err, SB_E_INVALID);
+    if (max_chunks == 0 || max_chunks > sbk::K11_MAX_CHUNKS) return fail(err, SB_E_INVALID, max_chunks, sbk::K11_MAX_CHUNKS);
+    if (batch->count == 0) { ok(err); return 0; }
+    const uint64_t tb = sbk::k14_tables_bytes(batch->count, max_chunks);
+    if (tables_bytes < tb) return fail(err, SB_E_INVALID, tables_bytes, tb);
+    const uint64_t need = table_batch_ws_bytes(batch->count, in_bytes, max_chunks);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_frame_table_build_batch(*c, *batch, in_bytes, flags, d_chunk_offs, d_index_at, max_chunks, d_tables,
+                                        d_table_offs, d_results, scratch, (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;

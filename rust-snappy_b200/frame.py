@@ -291,7 +291,8 @@ class RangeReader:
 
 class TableReader:
     """Random access to the decoded bytes of many frame streams on the device. Each stream gets a seek table, built once
-    on the device: a pointer-free list of its data chunks with their decoded offsets. `read_ranges([(i, lo, n), ...])`
+    on the device: a pointer-free list of its data chunks with their decoded offsets. The tables are built in batch
+    calls (sb_frame_table_build_batch_device_ws), one per group of streams whatever their number. `read_ranges([(i, lo, n), ...])`
     then serves ranges of any of the streams in one library call per group, decoding and checksumming only the chunks
     they cover, with no pass over any stream's headers. Every range gives what `RangeReader(streams[i]).read(lo, n)`
     gives. A stream is a bytes-like object (uploaded once) or a contiguous 1-D CUDA uint8 tensor (kept alive).
@@ -303,38 +304,107 @@ class TableReader:
     def __init__(self, streams, fragment=False):
         import numpy as np
         import torch
-        L = _lib.lib()
         self._dev = torch.device("cuda", torch.cuda.current_device())
         self._cuda = torch.cuda.current_stream(self._dev).cuda_stream
-        self._ins = []
+        self._ins, host = [], []
         for s in streams:
             if isinstance(s, torch.Tensor):
                 if not s.is_cuda or s.dtype != torch.uint8 or s.dim() != 1 or not s.is_contiguous():
                     raise ValueError("TableReader takes contiguous 1-D CUDA uint8 tensors")
                 self._ins.append(s)
             else:
-                self._ins.append(torch.from_numpy(np.frombuffer(s, dtype=np.uint8).copy()).to(self._dev))
+                host.append((len(self._ins), np.frombuffer(s, dtype=np.uint8)))
+                self._ins.append(None)
+        if host:                                                         # the bytes-like streams go up in one copy
+            at = np.cumsum([0] + [v.size for _, v in host])
+            cat = np.empty(int(at[-1]) + 1, dtype=np.uint8)
+            for (_, v), o in zip(host, at):
+                cat[o:o + v.size] = v
+            t_all = torch.from_numpy(cat).to(self._dev)
+            for (i, v), o in zip(host, at):
+                self._ins[i] = t_all[int(o):int(o) + v.size]
         flags = 1 if fragment else 0
         count = len(self._ins)
-        # the chunk table as RangeReader sizes it: encoder chunks hold 64 KiB, and any data chunk is at least 8 bytes
-        caps = [min(t.numel() // 1024 + 16, MAX_BATCH_CHUNKS) for t in self._ins]
-        tables, results = self._build(range(count), caps, flags)
-        redo = [i for i in range(count) if results[i].status.code == 202 and results[i].status.b == 1]
-        if redo:
-            for i in redo:
-                caps[i] = min(self._ins[i].numel() // 8 + 16, MAX_BATCH_CHUNKS)
-            more, res2 = self._build(redo, [caps[i] for i in redo], flags)
-            for j, i in enumerate(redo):
-                tables[i], results[i] = more[j], res2[j]
-        # keep each table at its exact size
-        self._tables = [t[:L.sb_frame_table_bytes(r.nchunks)].clone() for t, r in zip(tables, results)]
+        lens = [t.numel() for t in self._ins]
+        self._bufs = []                                                  # the tables live in these
+        ptrs, results = [0] * count, [None] * count
+        # a stream that fits an sb_batch unit is tabled in a batch call; a longer one gets a build of its own
+        for i, t, r in zip(*self._build([i for i in range(count) if lens[i] > 0xFFFFFFFF], flags)):
+            self._bufs.append(t)
+            ptrs[i], results[i] = t.data_ptr(), r
+        # the chunk table as RangeReader sizes it: encoder chunks hold 64 KiB, and any data chunk is at least 8 bytes.
+        # Streams that did not fit the first time are built again with the larger bound.
+        todo = [i for i in range(count) if lens[i] <= 0xFFFFFFFF]
+        for per in (1024, 8):
+            for i, p, r in self._build_batch(todo, [min(lens[i] // per + 16, MAX_BATCH_CHUNKS) for i in todo], flags):
+                ptrs[i], results[i] = p, r
+            todo = [i for i in todo if results[i].status.code == 202 and results[i].status.b == 1]
         self.lengths = [int(r.bytes) for r in results]
         to64 = lambda v: torch.from_numpy(np.array(v, dtype=np.uint64).view(np.int64)).to(self._dev)
-        self._t_tables = to64([t.data_ptr() for t in self._tables] + [0])
+        self._t_tables = to64(ptrs + [0])
         self._t_ins = to64([t.data_ptr() for t in self._ins] + [0])
-        self._t_lens = to64([t.numel() for t in self._ins] + [0])
+        self._t_lens = to64(lens + [0])
 
-    def _build(self, which, caps, flags):
+    def _build_batch(self, which, caps, flags):
+        """sb_frame_table_build_batch_device_ws over groups of streams whose chunk tables (caps) sum to at most
+        MAX_BATCH_CHUNKS: one call and one wait per group, whatever the number of streams. A group's tables stay in one
+        buffer cut to their packed size. Yields (stream, its table's address, its result) for every stream."""
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        groups, cur, total = [], [], 0
+        for i, c in zip(which, caps):
+            if cur and total + c > MAX_BATCH_CHUNKS:
+                groups.append((cur, total))
+                cur, total = [], 0
+            cur.append(i)
+            total += c
+        if cur:
+            groups.append((cur, total))
+        rsz = C.sizeof(_lib.SbFrameResult)
+        for g, max_chunks in groups:
+            k = len(g)
+            ins = [self._ins[i] for i in g]
+            in_bytes = sum(t.numel() for t in ins)
+            desc = np.concatenate([np.array([t.data_ptr() for t in ins], dtype=np.uint64).view(np.int64),
+                                   np.array([t.numel() for t in ins] + [0] * (k % 2), dtype=np.uint32).view(np.int64)])
+            t_desc = torch.from_numpy(desc).to(self._dev)
+            b = _lib.SbBatch()
+            b.in_ptrs, b.in_lens, b.count = t_desc.data_ptr(), t_desc.data_ptr() + 8 * k, k
+            tb = L.sb_frame_table_batch_bytes(k, max_chunks)
+            t_tab = torch.empty(tb, dtype=torch.uint8, device=self._dev)
+            t_res = torch.empty(8 * (k + 1) + rsz * k, dtype=torch.uint8, device=self._dev)   # offsets, then results
+            need = L.sb_frame_table_build_batch_scratch_bytes(k, in_bytes, max_chunks)
+            scr = torch.empty(need, dtype=torch.uint8, device=self._dev)
+            e = _lib.SbError()
+            if L.sb_frame_table_build_batch_device_ws(C.byref(b), in_bytes, flags, None, None, max_chunks,
+                                                      t_tab.data_ptr(), tb, t_res.data_ptr(),
+                                                      t_res.data_ptr() + 8 * (k + 1), scr.data_ptr(), need, self._cuda,
+                                                      C.byref(e)):
+                raise from_c(e)
+            back = t_res.cpu().numpy()
+            offs = back[:8 * (k + 1)].view(np.uint64)
+            kept = t_tab[:int(offs[k])].clone()
+            self._bufs.append(kept)
+            raw = back[8 * (k + 1):].tobytes()
+            for j, i in enumerate(g):
+                yield i, kept.data_ptr() + int(offs[j]), _lib.SbFrameResult.from_buffer_copy(raw[j * rsz:(j + 1) * rsz])
+
+    def _build(self, which, flags):
+        """A table per stream by sb_frame_table_build_device_ws (streams too long for a batch unit), its chunk table
+        sized as RangeReader sizes it and built once more when too small: (streams, tables cut to size, results)."""
+        L = _lib.lib()
+        if not which:
+            return [], [], []
+        caps = [min(self._ins[i].numel() // 1024 + 16, MAX_BATCH_CHUNKS) for i in which]
+        tables, results = self._build_each(which, caps, flags)
+        for j, i in enumerate(which):
+            if results[j].status.code == 202 and results[j].status.b == 1:
+                more, res2 = self._build_each([i], [min(self._ins[i].numel() // 8 + 16, MAX_BATCH_CHUNKS)], flags)
+                tables[j], results[j] = more[0], res2[0]
+        return which, [t[:L.sb_frame_table_bytes(r.nchunks)].clone() for t, r in zip(tables, results)], results
+
+    def _build_each(self, which, caps, flags):
         """One sb_frame_table_build_device_ws per stream, one wait for all: (tables, results)."""
         import numpy as np
         import torch
