@@ -405,6 +405,65 @@ int sb_frame_table_decode_ranges_device_ws(const void* const* d_tables, const ui
                                            uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
                                            uint64_t scratch_bytes, void* stream, sb_error* err);
 
+/* Seek tables of a batch of raw streams in one call, built from the 64 KiB block starts that
+ * sb_decompress_batch_device_ws finds, every block decoded and checksummed once. Unit i is batch input i (in_ptrs or
+ * in_base + stride, in_lens or the uniform length, count); the out_* fields, out_lens and statuses are not read. in_bytes
+ * means what it means for sb_decompress_batch_device_ws.
+ *   A raw table is a 64-byte header (a magic word with the format version, distinct from a frame table's; the stream's
+ *   compressed length n; the varint header length hl; the decoded length dn; the block count ceil(dn / 65536); a
+ *   seekable flag; the reason a stream is not seekable, for diagnostics only) and one 8-byte record per 64 KiB output
+ *   block: the compressed offset of the block's first element and the masked CRC-32C of its decoded bytes. Block j's
+ *   compressed bytes end where block j + 1's begin (n for the last); its decoded offset 65536 * j and length
+ *   min(65536, dn - 65536 * j) are implied. sb_raw_table_bytes(nblocks) = 64 + 8 * nblocks. A table holds no pointers and
+ *   may be copied or moved.
+ *   A unit is seekable when Decoder::decompress returns Ok and every block decodes alone to the same bytes: a unit
+ *   announcing more than 65,536 bytes that sb_decompress_batch_device_ws (same in_bytes, caps of at least dn) splits and
+ *   decodes block-parallel with Ok (d_unit_blocks[i] > 0), or a unit announcing at most 65,536 bytes (0 included) that
+ *   decodes Ok. Everything else (empty input, bad header, copies into an earlier block, elements across a block
+ *   boundary, unblocked encoders, corrupt or truncated streams, and units over one block when the lengths sum past
+ *   in_bytes) is not seekable.
+ *   The tables are packed back to back in batch order into d_tables (device, 8-byte aligned, at least
+ *   sb_raw_table_batch_bytes(count, in_bytes) bytes). d_table_offs (device, count + 1 entries) gets d_table_offs[0] = 0
+ *   and d_table_offs[i + 1] = d_table_offs[i] + sb_raw_table_bytes(d_results[i].nchunks). d_results[i] is {Ok, dn,
+ *   nblocks} for a seekable unit and {SB_E_INVALID{a=i, b=0, c=5}, 0, 0} otherwise; a unit that is not seekable gets a
+ *   64-byte header only. Every table is byte-identical (padding included) to what a count == 1 build of that stream gives.
+ * Scratch: sb_raw_table_build_batch_scratch_bytes(count, in_bytes), need not be zeroed. Stream ordered, no allocation, no
+ * host synchronisation, and the same launches whatever count holds. Null pointers, count >= 2^31 and tables or scratch
+ * that are too small are SB_E_INVALID with nothing launched; count == 0 does nothing. */
+uint64_t sb_raw_table_bytes(uint32_t nblocks);
+uint64_t sb_raw_table_batch_bytes(uint32_t count, uint64_t in_bytes);
+uint64_t sb_raw_table_build_batch_scratch_bytes(uint32_t count, uint64_t in_bytes);
+int sb_raw_table_build_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, void* d_tables, uint64_t tables_bytes,
+                                       uint64_t* d_table_offs, sb_frame_result* d_results, void* scratch,
+                                       uint64_t scratch_bytes, void* stream, sb_error* err);
+/* Byte ranges of many tabled raw streams in one call. The arguments mean what they mean for
+ * sb_frame_table_decode_ranges_device_ws: stream u is d_ins[u][0 .. d_in_lens[u]) and d_tables[u] its raw seek table, and
+ * range r asks for decoded bytes [d_lo[r], d_lo[r] + d_len[r]) of stream d_unit[r] into d_out_ptrs[r]. With
+ * end = min(lo + len, dn), a range decodes exactly the blocks that overlap [lo, end) and checks each one's CRC against its
+ * record. d_statuses[r] and d_out_lens[r], in priority order:
+ *   1. d_unit[r] >= count: SB_E_INVALID{a=unit, b=count, c=1}, 0;
+ *   2. d_tables[u] is not a raw table of this format, or was built over a stream of another length than d_in_lens[u]:
+ *      SB_E_INVALID{a=d_in_lens[u], b=the table's n (0 if it is not a raw table), c=2}, 0;
+ *   3. the stream is not seekable: SB_E_INVALID{a=u, b=0, c=5}, 0;
+ *   4. a covered block fails, the first in stream order j, with out_len max(65536 * j, lo) - lo: SB_E_INVALID{a=j, b=0,
+ *      c=3} when its record breaks the build's bounds (offsets non-decreasing, every block's bytes inside [hl, n), block
+ *      count ceil(dn / 65536), dn < 2^32), SB_E_INVALID{a=j, b=0, c=4} when it does not decode to its CRC (the stream is
+ *      not the one the table was built over);
+ *   5. otherwise Ok; max(end - lo, 0) (a range past the end is a short read, like pread).
+ *   For a seekable table built from stream S and read over S, every range is Ok and equals Decoder::decompress(S)[lo..end].
+ *   No table content makes the call read outside a stream or write outside [out_r, out_r + max(end - lo, 0)), the
+ *   staging or the scratch.
+ * A block shared by several ranges is decoded once per range; the scratch, sb_raw_table_ranges_scratch_bytes(nranges)
+ * bytes, holds 128 KiB of staging per range. Stream ordered, no allocation, no host synchronisation, and the same
+ * launches whatever count and nranges; nranges == 0 does nothing. Null pointers that are needed, count or
+ * nranges >= 2^31 and scratch that is too small are SB_E_INVALID with nothing launched. */
+uint64_t sb_raw_table_ranges_scratch_bytes(uint32_t nranges);
+int sb_raw_table_decode_ranges_device_ws(const void* const* d_tables, const uint8_t* const* d_ins,
+                                         const uint64_t* d_in_lens, uint32_t count, const uint32_t* d_unit,
+                                         const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                                         uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
+                                         uint64_t scratch_bytes, void* stream, sb_error* err);
+
 /* Chunk index of a frame stream in device memory, built in parallel on the device:
  * the offset of every chunk header in d_in[0..n) followed by n -- exactly the
  * d_chunk_offs that sb_frame_decode_device_ws accepts (max_chunks + 1 entries).

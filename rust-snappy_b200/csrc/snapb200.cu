@@ -27,6 +27,7 @@
 #include "k12_frame_range_decode.cuh"
 #include "k13_frame_table.cuh"
 #include "k14_frame_table_batch.cuh"
+#include "k15_raw_table.cuh"
 
 namespace {
 
@@ -122,6 +123,16 @@ __global__ void __launch_bounds__(128) k13_finish_kernel(sbk::TablePlan q) { sbk
 __global__ void __launch_bounds__(1024) k14_size_local_kernel(sbk::TableBatchPlan t) { sbk::k14_size_local_body(t); }
 __global__ void __launch_bounds__(1024) k14_size_tiles_kernel(sbk::TableBatchPlan t) { sbk::k14_size_tiles_body(t); }
 __global__ void __launch_bounds__(256) k14_export_kernel(sbk::TableBatchPlan t) { sbk::k14_export_body(t); }
+// with the occupancy hint ptxas keeps the block lookup in registers across K2 and K3 (without it: 48 and a 16-byte spill)
+__global__ void __launch_bounds__(128, 4) k15_validate_kernel(sbk::RawTableBuildPlan t) { sbk::k15_validate_body(t); }
+__global__ void __launch_bounds__(1024) k15_size_local_kernel(sbk::RawTableBuildPlan t) { sbk::k15_size_local_body(t); }
+__global__ void __launch_bounds__(1024) k15_size_tiles_kernel(sbk::RawTableBuildPlan t) { sbk::k15_size_tiles_body(t); }
+__global__ void __launch_bounds__(256) k15_export_kernel(sbk::RawTableBuildPlan t) { sbk::k15_export_body(t); }
+__global__ void __launch_bounds__(1024) k15_plan_kernel(sbk::RawRangePlan q) { sbk::k15_plan_body(q); }
+__global__ void __launch_bounds__(1024) k15_plan_tiles_kernel(sbk::RawRangePlan q) { sbk::k15_plan_tiles_body(q); }
+// K13's decode budget: 4 CTAs of 128 per SM at least
+__global__ void __launch_bounds__(128, 4) k15_decode_kernel(sbk::RawRangePlan q) { sbk::k15_decode_body(q); }
+__global__ void __launch_bounds__(256) k15_finish_kernel(sbk::RawRangePlan q) { sbk::k15_finish_body(q); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -548,24 +559,28 @@ int launch_raw_decode(Ctx& c, const sbk::RawPlan& p, cudaStream_t st, sb_error* 
 
 // ---- raw batch decode (K8 over every unit with more than one block, one warp for the rest)
 uint64_t raw_batch_ws_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k8b_carve(nullptr, count, in_bytes, nullptr); }
-int launch_raw_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_unit_blocks, void* scratch, cudaStream_t st,
-                     sb_error* err) {
-    if (b.count == 0) return 0;
+// grids over lists whose true lengths are on the device: at most `per_sm` CTAs per SM, grid-stride beyond that
+unsigned device_grid(const Ctx& c, uint64_t items, unsigned per_cta, unsigned per_sm) {
+    const uint64_t g = (items + per_cta - 1) / per_cta, most = (uint64_t)per_sm * c.sms;
+    return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most;
+}
+sbk::RawBatchPlan make_raw_batch_plan(const sb_batch& b, uint64_t in_bytes, uint32_t* d_unit_blocks, void* scratch) {
     sbk::RawBatchPlan q;
     memset(&q, 0, sizeof q);
     q.b = b; q.seg = sbk::k8_seg_len(k8_want_seg()); q.unit_blocks = d_unit_blocks;
     sbk::k8b_carve(scratch, b.count, in_bytes, &q);
-    // grids: warps over the segment / block / unit lists, whose true lengths are on the device
-    auto warps = [&](uint64_t n, unsigned per_sm) {
-        const uint64_t g = (n + 3) / 4, most = (uint64_t)per_sm * c.sms;
-        return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most;
-    };
-    const uint64_t in = q.in_bytes;
+    return q;
+}
+// K8b's split part, k8b_plan .. k8b_cuts: afterwards every split unit's control record and cut table are in the scratch.
+// Nothing here writes output: of the out fields only the caps are read.
+int raw_batch_split(Ctx& c, const sbk::RawBatchPlan& q, cudaStream_t st, sb_error* err) {
+    // grids: warps over the segment list, whose true length is on the device
+    const sb_batch& b = q.b;
     CK(cudaMemsetAsync(q.bctl, 0, sizeof(sbk::RawBatchCtl), st));
     const unsigned utiles = (unsigned)(((uint64_t)b.count + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
     k8b_plan_kernel<<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
     k8b_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
-    const unsigned segw = warps(q.nseg_cap, 16);
+    const unsigned segw = device_grid(c, q.nseg_cap, 4, 16);
     k8b_chains_kernel<<<segw, 128, 0, st>>>(q);
     k8b_merge_kernel<<<segw, 128, 0, st>>>(q);
     const unsigned sgrid = b.count < (uint32_t)(8 * c.sms) ? b.count : (unsigned)(8 * c.sms);
@@ -575,11 +590,22 @@ int launch_raw_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_u
     k8b_scan_local_kernel<<<ctiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
     k8b_scan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
     k8b_cuts_kernel<<<segw, 128, 0, st>>>(q);
-    k8b_blocks_kernel<<<warps(in / 3072 + b.count, 16), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
-    // the one-warp pass, sized like launch_k2
+    g_launches += 9;
+    CK(cudaGetLastError());
+    return 0;
+}
+int launch_raw_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_unit_blocks, void* scratch, cudaStream_t st,
+                     sb_error* err) {
+    if (b.count == 0) return 0;
+    const sbk::RawBatchPlan q = make_raw_batch_plan(b, in_bytes, d_unit_blocks, scratch);
+    int rc = raw_batch_split(c, q, st, err);
+    if (rc) return rc;
+    // the payload part: warps over the block list, whose true length is on the device, then the one-warp pass, sized
+    // like launch_k2
+    k8b_blocks_kernel<<<device_grid(c, q.in_bytes / 3072 + b.count, 4, 16), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
     static const int per_sm = getenv("SNAPB200_K2_CTAS") ? atoi(getenv("SNAPB200_K2_CTAS")) : K2_DEFAULT_CTAS_PER_SM;
-    k8b_finish_kernel<<<warps(b.count, per_sm), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
-    g_launches += 11;
+    k8b_finish_kernel<<<device_grid(c, b.count, 4, per_sm), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    g_launches += 2;
     CK(cudaGetLastError());
     return 0;
 }
@@ -651,11 +677,6 @@ int launch_frame_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint64_t* d
 // ---- frame batch decode (K7's index or a walk per unit, K5's parse, decode and CRC over all units' chunks)
 uint64_t frame_decode_batch_ws_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks) {
     return sbk::k11_carve(nullptr, count, in_bytes, max_chunks, nullptr);
-}
-// grids over lists whose true lengths are on the device: at most `per_sm` CTAs per SM, grid-stride beyond that
-unsigned device_grid(const Ctx& c, uint64_t items, unsigned per_cta, unsigned per_sm) {
-    const uint64_t g = (items + per_cta - 1) / per_cta, most = (uint64_t)per_sm * c.sms;
-    return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most;
 }
 sbk::FrameDecodeBatchPlan make_frame_decode_batch_plan(const sb_batch& b, uint64_t in_bytes, uint32_t flags,
                                                        const uint64_t* d_chunk_offs, const uint64_t* d_index_at,
@@ -790,6 +811,42 @@ int launch_frame_table_ranges(Ctx& c, const sbk::TablePlan& q, cudaStream_t st, 
     k13_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
     k13_decode_kernel<<<(unsigned)most, 128, smem + 4 * sizeof(sb_error), st>>>(q);
     k13_finish_kernel<<<fw < most ? (unsigned)fw : (unsigned)most, 128, smem, st>>>(q);
+    g_launches += 4;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// ---- raw seek tables of a batch (K8b's split part, then K15's validation, size scan and export) and ranges over
+// tabled raw streams (K15)
+int launch_raw_table_build_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, void* d_tables, uint64_t* d_table_offs,
+                                 sb_frame_result* d_results, void* scratch, cudaStream_t st, sb_error* err) {
+    sb_batch u;                                                      // the inputs only, with a cap no header exceeds
+    memset(&u, 0, sizeof u);
+    u.in_ptrs = b.in_ptrs; u.in_base = b.in_base; u.in_stride = b.in_stride; u.in_lens = b.in_lens;
+    u.in_len_uniform = b.in_len_uniform; u.out_cap_uniform = 0xFFFFFFFFu; u.count = b.count;
+    sbk::RawTableBuildPlan t;
+    memset(&t, 0, sizeof t);
+    t.q = make_raw_batch_plan(u, in_bytes, nullptr, scratch);
+    sbk::k15_carve(scratch, b.count, in_bytes, &t);
+    t.tables = (uint8_t*)d_tables; t.table_offs = d_table_offs; t.results = d_results;
+    int rc = raw_batch_split(c, t.q, st, err);
+    if (rc) return rc;
+    const unsigned utiles = (unsigned)(((uint64_t)b.count + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    k15_validate_kernel<<<(t.nslots + 3) / 4, 128, sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP, st>>>(t);
+    k15_size_local_kernel<<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(t);
+    k15_size_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(t);
+    k15_export_kernel<<<device_grid(c, sbk::k15_blocks_bound(b.count, in_bytes) + b.count + 1, 256, 16), 256, 0, st>>>(t);
+    g_launches += 4;
+    CK(cudaGetLastError());
+    return 0;
+}
+int launch_raw_table_ranges(Ctx& c, const sbk::RawRangePlan& q, cudaStream_t st, sb_error* err) {
+    // the pair total is on the device: 4 warps per CTA, at most 16 CTAs per SM, grid-stride beyond that
+    const unsigned ptiles = (unsigned)(((uint64_t)q.nranges + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    k15_plan_kernel<<<ptiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k15_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    k15_decode_kernel<<<16 * c.sms, 128, sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    k15_finish_kernel<<<device_grid(c, q.nranges, 256, 16), 256, 0, st>>>(q);
     g_launches += 4;
     CK(cudaGetLastError());
     return 0;
@@ -1079,6 +1136,59 @@ int sb_frame_table_decode_ranges_device_ws(const void* const* d_tables, const ui
     q.unit = d_unit; q.lo = d_lo; q.len = d_len; q.outs = d_out_ptrs; q.out_lens = d_out_lens; q.statuses = d_statuses;
     sbk::k13_carve(scratch, nranges, &q);
     rc = launch_frame_table_ranges(*c, q, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_raw_table_bytes(uint32_t nblocks) { return sbk::k15_table_bytes(nblocks); }
+uint64_t sb_raw_table_batch_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k15_tables_bytes(count, in_bytes); }
+uint64_t sb_raw_table_build_batch_scratch_bytes(uint32_t count, uint64_t in_bytes) {
+    return sbk::k15_carve(nullptr, count, in_bytes, nullptr);
+}
+
+int sb_raw_table_build_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, void* d_tables, uint64_t tables_bytes,
+                                       uint64_t* d_table_offs, sb_frame_result* d_results, void* scratch,
+                                       uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if (!batch || !d_tables || !d_table_offs || !d_results || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K8B_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K8B_MAX_COUNT);
+    if (batch->count == 0) { ok(err); return 0; }
+    const uint64_t tb = sbk::k15_tables_bytes(batch->count, in_bytes);
+    if (tables_bytes < tb) return fail(err, SB_E_INVALID, tables_bytes, tb);
+    const uint64_t need = sbk::k15_carve(nullptr, batch->count, in_bytes, nullptr);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_raw_table_build_batch(*c, *batch, in_bytes, d_tables, d_table_offs, d_results, scratch, (cudaStream_t)stream,
+                                      err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_raw_table_ranges_scratch_bytes(uint32_t nranges) { return sbk::k15_ranges_carve(nullptr, nranges, nullptr); }
+
+int sb_raw_table_decode_ranges_device_ws(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens,
+                                         uint32_t count, const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len,
+                                         uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
+                                         uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if (count >= sbk::K15_MAX_COUNT) return fail(err, SB_E_INVALID, count, sbk::K15_MAX_COUNT);
+    if (nranges >= sbk::K12_MAX_RANGES) return fail(err, SB_E_INVALID, nranges, sbk::K12_MAX_RANGES);
+    if (nranges == 0) { ok(err); return 0; }
+    if (count && (!d_tables || !d_ins || !d_in_lens)) return fail(err, SB_E_INVALID);
+    if (!d_unit || !d_lo || !d_len || !d_out_ptrs || !d_out_lens || !d_statuses || !scratch) return fail(err, SB_E_INVALID);
+    const uint64_t need = sbk::k15_ranges_carve(nullptr, nranges, nullptr);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    sbk::RawRangePlan q;
+    memset(&q, 0, sizeof q);
+    q.tables = d_tables; q.ins = d_ins; q.in_lens = d_in_lens; q.count = count;
+    q.unit = d_unit; q.lo = d_lo; q.len = d_len; q.outs = d_out_ptrs; q.out_lens = d_out_lens; q.statuses = d_statuses;
+    sbk::k15_ranges_carve(scratch, nranges, &q);
+    rc = launch_raw_table_ranges(*c, q, (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;

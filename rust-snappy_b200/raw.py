@@ -76,3 +76,218 @@ def crc32c_masked(data) -> int:
     if _lib.lib().sb_crc32c_masked(p, len(data), C.byref(out), C.byref(e)):
         raise from_c(e)
     return out.value
+
+
+class TableReader:
+    """Random access to the decoded bytes of many raw streams on the device. Each stream gets a seek table, built once on
+    the device in batch calls (sb_raw_table_build_batch_device_ws), one per group of streams whatever their number: the
+    compressed offset and CRC of every 64 KiB output block, every block decoded and checksummed once. `read_ranges([(i,
+    lo, n), ...])` then serves ranges of any of the streams in one library call per group, decoding and checksumming only
+    the blocks they cover. Every range gives `Decoder().decompress_vec(streams[i])[lo:lo + n]`. A stream that is not
+    seekable (see `seekable`: not block-independent, or not decodable) is decoded whole on the device for each call
+    that reads it, and gives exactly that slice or raises that call's error. A stream is a bytes-like object (uploaded
+    with the others in one copy) or a contiguous 1-D CUDA uint8 tensor (kept alive), of at most 2^32 - 1 bytes. Calls run
+    on the current torch stream and wait for their results."""
+
+    RANGES_PER_CALL = 4096                    # 128 KiB of staging per range: 512 MiB per call at most
+    BYTES_PER_CALL = 1 << 30                  # output bytes one call gathers (a single larger range gets its own call)
+    GROUP_BYTES = 1 << 34                     # compressed bytes one build call takes (its scratch grows with them)
+
+    def __init__(self, streams):
+        import numpy as np
+        import torch
+        self._dev = torch.device("cuda", torch.cuda.current_device())
+        self._cuda = torch.cuda.current_stream(self._dev).cuda_stream
+        self._ins, host = [], []
+        for s in streams:
+            if isinstance(s, torch.Tensor):
+                if not s.is_cuda or s.dtype != torch.uint8 or s.dim() != 1 or not s.is_contiguous():
+                    raise ValueError("TableReader takes contiguous 1-D CUDA uint8 tensors")
+                self._ins.append(s)
+            else:
+                host.append((len(self._ins), np.frombuffer(s, dtype=np.uint8)))
+                self._ins.append(None)
+        for i, v in host:
+            if v.size > 0xFFFFFFFF:
+                raise ValueError("stream %d has %d bytes; a raw stream has at most 2^32 - 1" % (i, v.size))
+        if host:                                                         # the bytes-like streams go up in one copy
+            at = np.cumsum([0] + [v.size for _, v in host])
+            cat = np.empty(int(at[-1]) + 1, dtype=np.uint8)
+            for (_, v), o in zip(host, at):
+                cat[o:o + v.size] = v
+            t_all = torch.from_numpy(cat).to(self._dev)
+            for (i, v), o in zip(host, at):
+                self._ins[i] = t_all[int(o):int(o) + v.size]
+        lens = [t.numel() for t in self._ins]
+        for i, n in enumerate(lens):
+            if n > 0xFFFFFFFF:
+                raise ValueError("stream %d has %d bytes; a raw stream has at most 2^32 - 1" % (i, n))
+        count = len(self._ins)
+        self._bufs = []                                                  # the tables live in these
+        ptrs, results = [0] * count, [None] * count
+        for i, p, r in self._build(list(range(count))):
+            ptrs[i], results[i] = p, r
+        self.seekable = [r.status.code == 0 for r in results]
+        self.lengths = [int(r.bytes) if ok else None for r, ok in zip(results, self.seekable)]
+        to64 = lambda v: torch.from_numpy(np.array(v, dtype=np.uint64).view(np.int64)).to(self._dev)
+        self._t_tables = to64(ptrs + [0])
+        self._t_ins = to64([t.data_ptr() for t in self._ins] + [0])
+        self._t_lens = to64(lens + [0])
+
+    def _build(self, which):
+        """sb_raw_table_build_batch_device_ws over groups of at most GROUP_BYTES compressed bytes: one call and one wait
+        per group. A group's tables stay in one buffer cut to their packed size. Yields (stream, its table's address, its
+        result) for every stream."""
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        groups, cur, total = [], [], 0
+        for i in which:
+            n = self._ins[i].numel()
+            if cur and total + n > self.GROUP_BYTES:
+                groups.append(cur)
+                cur, total = [], 0
+            cur.append(i)
+            total += n
+        if cur:
+            groups.append(cur)
+        rsz = C.sizeof(_lib.SbFrameResult)
+        for g in groups:
+            k = len(g)
+            ins = [self._ins[i] for i in g]
+            in_bytes = sum(t.numel() for t in ins)
+            desc = np.concatenate([np.array([t.data_ptr() for t in ins], dtype=np.uint64).view(np.int64),
+                                   np.array([t.numel() for t in ins] + [0] * (k % 2), dtype=np.uint32).view(np.int64)])
+            t_desc = torch.from_numpy(desc).to(self._dev)
+            b = _lib.SbBatch()
+            b.in_ptrs, b.in_lens, b.count = t_desc.data_ptr(), t_desc.data_ptr() + 8 * k, k
+            tb = L.sb_raw_table_batch_bytes(k, in_bytes)
+            t_tab = torch.empty(tb, dtype=torch.uint8, device=self._dev)
+            t_res = torch.empty(8 * (k + 1) + rsz * k, dtype=torch.uint8, device=self._dev)   # offsets, then results
+            need = L.sb_raw_table_build_batch_scratch_bytes(k, in_bytes)
+            scr = torch.empty(need, dtype=torch.uint8, device=self._dev)
+            e = _lib.SbError()
+            if L.sb_raw_table_build_batch_device_ws(C.byref(b), in_bytes, t_tab.data_ptr(), tb, t_res.data_ptr(),
+                                                    t_res.data_ptr() + 8 * (k + 1), scr.data_ptr(), need, self._cuda,
+                                                    C.byref(e)):
+                raise from_c(e)
+            back = t_res.cpu().numpy()
+            offs = back[:8 * (k + 1)].view(np.uint64)
+            kept = t_tab[:int(offs[k])].clone()
+            self._bufs.append(kept)
+            raw = back[8 * (k + 1):].tobytes()
+            for j, i in enumerate(g):
+                yield i, kept.data_ptr() + int(offs[j]), _lib.SbFrameResult.from_buffer_copy(raw[j * rsz:(j + 1) * rsz])
+
+    def __len__(self):
+        return len(self._ins)
+
+    def _call(self, ranges):
+        """One sb_raw_table_decode_ranges_device_ws call: (out_lens, statuses, output tensor, offsets)."""
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        k = len(ranges)
+        room = [max(0, min(n, self.lengths[i] - lo)) for i, lo, n in ranges]
+        offs = np.zeros(k, dtype=np.int64)
+        if k:
+            offs[1:] = np.cumsum(room[:-1])
+        t_out = torch.empty(sum(room) + 1, dtype=torch.uint8, device=self._dev)
+        desc = np.array([lo for _, lo, _ in ranges] + [n for _, _, n in ranges], dtype=np.uint64).view(np.int64)
+        units = np.array([i for i, _, _ in ranges] + [0], dtype=np.uint32).view(np.int32)
+        t_desc = torch.from_numpy(np.concatenate([desc, offs + t_out.data_ptr()])).to(self._dev)
+        t_unit = torch.from_numpy(units).to(self._dev)
+        t_res = torch.zeros(5 * k, dtype=torch.int64, device=self._dev)       # out_lens, statuses
+        need = L.sb_raw_table_ranges_scratch_bytes(k)
+        scr = torch.empty(need, dtype=torch.uint8, device=self._dev)
+        e = _lib.SbError()
+        p = t_desc.data_ptr()
+        if L.sb_raw_table_decode_ranges_device_ws(self._t_tables.data_ptr(), self._t_ins.data_ptr(),
+                                                  self._t_lens.data_ptr(), len(self._ins), t_unit.data_ptr(), p, p + 8 * k,
+                                                  p + 16 * k, t_res.data_ptr(), t_res.data_ptr() + 8 * k, k,
+                                                  scr.data_ptr(), need, self._cuda, C.byref(e)):
+            raise from_c(e)
+        back = t_res.cpu().numpy().view(np.uint64)
+        return back[:k], back[k:5 * k].reshape(k, 4), t_out, offs
+
+    def _decode_whole(self, which):
+        """Streams that are not seekable, each as Decoder().decompress_vec gives it: {stream: bytes or the exception},
+        the decodable ones in one sb_decompress_batch_device_ws call."""
+        import numpy as np
+        import torch
+        L = _lib.lib()
+        got, todo = {}, []
+        for i in which:
+            try:                                                          # decompress_vec sizes its buffer this way
+                todo.append((i, decompress_len(self._ins[i][:10].cpu().numpy().tobytes())))
+            except Exception as x:
+                got[i] = x
+        if not todo:
+            return got
+        k = len(todo)
+        caps = [dn for _, dn in todo]
+        at = np.zeros(k, dtype=np.int64)
+        at[1:] = np.cumsum(caps[:-1])
+        t_out = torch.empty(sum(caps) + 1, dtype=torch.uint8, device=self._dev)
+        ins = [self._ins[i] for i, _ in todo]
+        desc = np.concatenate([np.array([t.data_ptr() for t in ins], dtype=np.uint64).view(np.int64), at + t_out.data_ptr(),
+                               np.array([t.numel() for t in ins] + caps, dtype=np.uint32).view(np.int64)])
+        t_desc = torch.from_numpy(desc).to(self._dev)
+        t_res = torch.zeros(k + 4 * k, dtype=torch.int64, device=self._dev)   # out_lens (u32), statuses
+        b = _lib.SbBatch()
+        p = t_desc.data_ptr()
+        b.in_ptrs, b.out_ptrs, b.in_lens, b.out_caps = p, p + 8 * k, p + 16 * k, p + 20 * k
+        b.out_lens, b.statuses, b.count = t_res.data_ptr(), t_res.data_ptr() + 8 * k, k
+        in_bytes = sum(t.numel() for t in ins)
+        need = L.sb_decompress_batch_scratch_bytes(k, in_bytes)
+        scr = torch.empty(need, dtype=torch.uint8, device=self._dev)
+        e = _lib.SbError()
+        if L.sb_decompress_batch_device_ws(C.byref(b), in_bytes, None, scr.data_ptr(), need, self._cuda, C.byref(e)):
+            raise from_c(e)
+        st = t_res.cpu().numpy().view(np.uint64)[k:].reshape(k, 4)
+        back = t_out.cpu().numpy()
+        for j, (i, dn) in enumerate(todo):
+            s = st[j]
+            got[i] = from_c(_lib.SbError(int(s[0] & 0xFFFFFFFF), 0, int(s[1]), int(s[2]), int(s[3]))) \
+                if s[0] & 0xFFFFFFFF else back[at[j]:at[j] + dn].tobytes()
+        return got
+
+    def read(self, i: int, lo: int, n: int) -> bytes:
+        """Decoded bytes [lo, lo + n) of stream i, fewer at the end of the stream."""
+        return self.read_ranges([(i, lo, n)])[0]
+
+    def read_ranges(self, ranges) -> list:
+        """One bytes object per (i, lo, n) range of stream i. Ranges may mix streams in any order and be empty,
+        unsorted, overlapping or repeated; each library call takes a group of them whose staging and output stay
+        bounded. Raises the first failing range's error."""
+        ranges = [(int(i), int(lo), int(n)) for i, lo, n in ranges]
+        for i, lo, n in ranges:
+            if not 0 <= i < len(self._ins):
+                raise IndexError("stream %d of %d" % (i, len(self._ins)))
+            if lo < 0 or n < 0 or lo + n > 0xFFFFFFFFFFFFFFFF:
+                raise ValueError("range (%d, %d) is not within 64-bit offsets" % (lo, n))
+        whole = self._decode_whole(sorted({i for i, _, _ in ranges if not self.seekable[i]}))
+        tabled = [r for r in ranges if self.seekable[r[0]]]
+        got, a = [], 0
+        while a < len(tabled):
+            b, size = a, 0
+            while b < len(tabled) and b - a < self.RANGES_PER_CALL:
+                i, lo, n = tabled[b]
+                room = max(0, min(n, self.lengths[i] - lo))
+                if b > a and size + room > self.BYTES_PER_CALL:
+                    break
+                size += room
+                b += 1
+            lens, sts, t_out, offs = self._call(tabled[a:b])
+            back = t_out.cpu().numpy()
+            for s, o, m in zip(sts, offs, lens):
+                got.append(from_c(_lib.SbError(int(s[0] & 0xFFFFFFFF), 0, int(s[1]), int(s[2]), int(s[3])))
+                           if s[0] & 0xFFFFFFFF else back[o:o + int(m)].tobytes())
+            a = b
+        out, it = [], iter(got)
+        for i, lo, n in ranges:
+            r = next(it) if self.seekable[i] else whole[i]
+            if isinstance(r, Exception):
+                raise r
+            out.append(r[lo:lo + n] if not self.seekable[i] else r)
+        return out
