@@ -464,6 +464,40 @@ int sb_raw_table_decode_ranges_device_ws(const void* const* d_tables, const uint
                                          uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
                                          uint64_t scratch_bytes, void* stream, sb_error* err);
 
+/* Batch encoders that also write one seek table per unit, so what they write is seekable without a build. Each does
+ * exactly what its untabled call does: output bytes, out_lens, statuses and (frame) d_chunk_offs are byte-identical to
+ * sb_compress_batch_device_ws / sb_frame_encode_batch_device_ws with the same arguments, rejected units and the in_bytes
+ * overflow (SB_E_INVALID{sum, in_bytes}) included. The tables are packed back to back in batch order into d_tables
+ * (device, 8-byte aligned, at least sb_compress_tables_bytes / sb_frame_encode_tables_bytes(count, in_bytes) bytes);
+ * d_table_offs (device, count + 1 entries) gets d_table_offs[0] = 0 and every table's end.
+ *   Raw: unit i's table and d_results[i] are byte-identical, padding included, to what sb_raw_table_build_batch_device_ws
+ *     (in_bytes at least the sum of out_lens) writes for out_i[0 .. out_lens[i]): {Ok, n, ceil(n / 65536)} and a seekable
+ *     table for every written unit; a rejected unit (0 bytes) gets the not-seekable header with n = 0 and
+ *     {SB_E_INVALID{a=i, b=0, c=5}, 0, 0}. One exception: a stream the build declines only because a K8 segment needs
+ *     more than 1,024 merge elements (reason 3). There the encoder's table is still seekable and correct, since the
+ *     encoder knows its own block starts.
+ *   Frame: unit i's table and d_results[i] are byte-identical to what sb_frame_table_build_batch_device_ws (flags 0, a
+ *     large enough max_chunks) writes for out_i[0 .. out_lens[i]). Empty and rejected units (0 bytes) get the table of
+ *     an empty stream.
+ * The records come from the encode itself: every block's compressed offset is a scan value of the encode, its decoded
+ * offset is 65536 * j and its masked CRC-32C comes from the compress kernel's emitter warp. No output is read back.
+ * Scratch: sb_compress_batch_tabled_scratch_bytes / sb_frame_encode_batch_tabled_scratch_bytes(count, in_bytes), need
+ * not be zeroed. Stream ordered, no allocation, no host synchronisation, and the same launches whatever count holds (for
+ * the frame call: one number with d_chunk_offs, one without). Null pointers (batch, out_lens, d_tables, d_table_offs,
+ * d_results, scratch), count >= 2^31, a bound whose block count does not fit one launch and tables or scratch that are
+ * too small are SB_E_INVALID with nothing launched; count == 0 does nothing. */
+uint64_t sb_compress_tables_bytes(uint32_t count, uint64_t in_bytes);
+uint64_t sb_compress_batch_tabled_scratch_bytes(uint32_t count, uint64_t in_bytes);
+int sb_compress_batch_tabled_device_ws(const sb_batch* batch, uint64_t in_bytes, void* d_tables, uint64_t tables_bytes,
+                                       uint64_t* d_table_offs, sb_frame_result* d_results, void* scratch,
+                                       uint64_t scratch_bytes, void* stream, sb_error* err);
+uint64_t sb_frame_encode_tables_bytes(uint32_t count, uint64_t in_bytes);
+uint64_t sb_frame_encode_batch_tabled_scratch_bytes(uint32_t count, uint64_t in_bytes);
+int sb_frame_encode_batch_tabled_device_ws(const sb_batch* batch, uint64_t in_bytes, uint64_t* d_chunk_offs,
+                                           void* d_tables, uint64_t tables_bytes, uint64_t* d_table_offs,
+                                           sb_frame_result* d_results, void* scratch, uint64_t scratch_bytes,
+                                           void* stream, sb_error* err);
+
 /* Chunk index of a frame stream in device memory, built in parallel on the device:
  * the offset of every chunk header in d_in[0..n) followed by n -- exactly the
  * d_chunk_offs that sb_frame_decode_device_ws accepts (max_chunks + 1 entries).

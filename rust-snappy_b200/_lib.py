@@ -46,6 +46,8 @@ SYMBOLS = [
     "sb_frame_table_batch_bytes", "sb_frame_table_build_batch_scratch_bytes", "sb_frame_table_build_batch_device_ws",
     "sb_raw_table_bytes", "sb_raw_table_batch_bytes", "sb_raw_table_build_batch_scratch_bytes",
     "sb_raw_table_build_batch_device_ws", "sb_raw_table_ranges_scratch_bytes", "sb_raw_table_decode_ranges_device_ws",
+    "sb_compress_tables_bytes", "sb_compress_batch_tabled_scratch_bytes", "sb_compress_batch_tabled_device_ws",
+    "sb_frame_encode_tables_bytes", "sb_frame_encode_batch_tabled_scratch_bytes", "sb_frame_encode_batch_tabled_device_ws",
     "sb_frame_max_len", "sb_frame_encode", "sb_frame_encode_ex", "sb_frame_decode", "sb_frame_encode_device",
     "sb_frame_encode_scratch_bytes", "sb_frame_encode_device_ws", "sb_frame_decode_scratch_bytes",
     "sb_frame_decode_device_ws", "sb_frame_decode_device", "sb_frame_index_scratch_bytes", "sb_frame_index_device_ws",
@@ -131,6 +133,14 @@ def lib():
     L.sb_raw_table_ranges_scratch_bytes.argtypes = [C.c_uint32]
     L.sb_raw_table_decode_ranges_device_ws.argtypes = [vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, C.c_uint32, vp,
                                                        C.c_uint64, vp, ep]
+    for name in ("sb_compress_tables_bytes", "sb_compress_batch_tabled_scratch_bytes", "sb_frame_encode_tables_bytes",
+                 "sb_frame_encode_batch_tabled_scratch_bytes"):
+        getattr(L, name).restype = C.c_uint64
+        getattr(L, name).argtypes = [C.c_uint32, C.c_uint64]
+    L.sb_compress_batch_tabled_device_ws.argtypes = [C.POINTER(SbBatch), C.c_uint64, vp, C.c_uint64, vp, vp, vp, C.c_uint64,
+                                                     vp, ep]
+    L.sb_frame_encode_batch_tabled_device_ws.argtypes = [C.POINTER(SbBatch), C.c_uint64, vp, vp, C.c_uint64, vp, vp, vp,
+                                                         C.c_uint64, vp, ep]
     L.sb_crc32c_masked_batch_device.argtypes = [C.POINTER(SbBatch), vp, ep]
     L.sb_frame_encode.argtypes = [vp, sz, vp, sz, szp, ep]
     L.sb_frame_encode_ex.argtypes = [vp, sz, vp, sz, szp, C.c_int, ep]

@@ -28,6 +28,7 @@
 #include "k13_frame_table.cuh"
 #include "k14_frame_table_batch.cuh"
 #include "k15_raw_table.cuh"
+#include "k16_encode_tables.cuh"
 
 namespace {
 
@@ -133,6 +134,11 @@ __global__ void __launch_bounds__(1024) k15_plan_tiles_kernel(sbk::RawRangePlan 
 // K13's decode budget: 4 CTAs of 128 per SM at least
 __global__ void __launch_bounds__(128, 4) k15_decode_kernel(sbk::RawRangePlan q) { sbk::k15_decode_body(q); }
 __global__ void __launch_bounds__(256) k15_finish_kernel(sbk::RawRangePlan q) { sbk::k15_finish_body(q); }
+template <bool FRAME>
+__global__ void __launch_bounds__(1024) k16_size_local_kernel(sbk::EncodeTablesPlan t) { sbk::k16_size_local_body<FRAME>(t); }
+__global__ void __launch_bounds__(1024) k16_size_tiles_kernel(sbk::EncodeTablesPlan t) { sbk::k16_size_tiles_body(t); }
+__global__ void __launch_bounds__(256) k16_raw_export_kernel(sbk::EncodeTablesPlan t) { sbk::k16_raw_export_body(t); }
+__global__ void __launch_bounds__(256) k16_frame_export_kernel(sbk::EncodeTablesPlan t) { sbk::k16_frame_export_body(t); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -613,11 +619,9 @@ int launch_raw_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_u
 
 // ---- raw batch compress (units of any length: every block of the batch in one K1 launch, assembled per unit)
 uint64_t raw_compress_ws_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k9_carve(nullptr, count, in_bytes, nullptr); }
-int launch_raw_compress(Ctx& c, const sb_batch& b, uint64_t in_bytes, void* scratch, cudaStream_t st, sb_error* err) {
-    sbk::RawCompressPlan q;
-    memset(&q, 0, sizeof q);
-    q.b = b;
-    sbk::k9_carve(scratch, b.count, in_bytes, &q);
+// K9's launch sequence over a carved plan; crcs: K1's masked CRC per entry (null: none, as the untabled call)
+int raw_compress_launches(Ctx& c, const sbk::RawCompressPlan& q, uint32_t* crcs, cudaStream_t st, sb_error* err) {
+    const sb_batch& b = q.b;
     auto threads = [](uint64_t n, unsigned per) { return (unsigned)((n + per - 1) / per); };
     CK(cudaMemsetAsync(q.ctl, 0, sizeof(sbk::RawCompressCtl), st));
     k9_plan_kernel<<<threads(b.count, 256), 256, 0, st>>>(q);
@@ -626,7 +630,7 @@ int launch_raw_compress(Ctx& c, const sb_batch& b, uint64_t in_bytes, void* scra
     k9_fill_kernel<<<threads(q.nk, 256), 256, 0, st>>>(q);
     g_launches += 4;
     CK(cudaGetLastError());
-    int rc = launch_k1(c, sbk::k9_k1_batch(q), 0u, nullptr, st, err);
+    int rc = launch_k1(c, sbk::k9_k1_batch(q), 0u, crcs, st, err);
     if (rc) return rc;
     k9_bscan_local_kernel<<<threads((uint64_t)q.nslot + 1, sbk::K4_TILE), sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
     k9_bscan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
@@ -638,15 +642,20 @@ int launch_raw_compress(Ctx& c, const sb_batch& b, uint64_t in_bytes, void* scra
     CK(cudaGetLastError());
     return 0;
 }
+int launch_raw_compress(Ctx& c, const sb_batch& b, uint64_t in_bytes, void* scratch, cudaStream_t st, sb_error* err) {
+    sbk::RawCompressPlan q;
+    memset(&q, 0, sizeof q);
+    q.b = b;
+    sbk::k9_carve(scratch, b.count, in_bytes, &q);
+    return raw_compress_launches(c, q, nullptr, st, err);
+}
 
 // ---- frame batch encode (K9's plan and slots, K1 in frame mode, frame chunks assembled per unit)
 uint64_t frame_batch_ws_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k10_carve(nullptr, count, in_bytes, nullptr); }
-int launch_frame_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint64_t* d_chunk_offs, void* scratch, cudaStream_t st,
-                       sb_error* err) {
-    sbk::FrameBatchPlan q;
-    memset(&q, 0, sizeof q);
-    q.r.b = b; q.idx = d_chunk_offs;
-    sbk::k10_carve(scratch, b.count, in_bytes, &q);
+// K10's launch sequence over a carved plan
+int frame_batch_launches(Ctx& c, const sbk::FrameBatchPlan& q, cudaStream_t st, sb_error* err) {
+    const sb_batch& b = q.r.b;
+    const uint64_t* d_chunk_offs = q.idx;
     auto threads = [](uint64_t n, unsigned per) { return (unsigned)((n + per - 1) / per); };
     // warp-per-item kernels: 8 warps per CTA, at most 16 CTAs per SM, grid-stride beyond that
     auto warps = [&](uint64_t n) { const uint64_t g = (n + 7) / 8, most = (uint64_t)16 * c.sms; return g == 0 ? 1u : g < most ? (unsigned)g : (unsigned)most; };
@@ -670,6 +679,57 @@ int launch_frame_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint64_t* d
     k10_gather_kernel<<<warps(q.r.nslot), 256, 0, st>>>(q);
     k10_finish_kernel<<<warps(b.count), 256, 0, st>>>(q);
     g_launches += 4;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+int launch_frame_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint64_t* d_chunk_offs, void* scratch, cudaStream_t st,
+                       sb_error* err) {
+    sbk::FrameBatchPlan q;
+    memset(&q, 0, sizeof q);
+    q.r.b = b; q.idx = d_chunk_offs;
+    sbk::k10_carve(scratch, b.count, in_bytes, &q);
+    return frame_batch_launches(c, q, st, err);
+}
+
+// ---- seek tables written by the batch encoders (K9 with K1's CRCs, or K10; then K16's size scan and export)
+uint64_t raw_tabled_ws_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k16_raw_carve(nullptr, count, in_bytes, nullptr); }
+uint64_t frame_tabled_ws_bytes(uint32_t count, uint64_t in_bytes) {
+    return sbk::k16_frame_carve(nullptr, count, in_bytes, nullptr);
+}
+// the checks both tabled encoders share; 0 when the call goes ahead, -1 for count == 0 (nothing to do, Ok)
+int tabled_checks(const sb_batch* batch, uint64_t in_bytes, bool frame, void* d_tables, uint64_t tables_bytes,
+                  uint64_t* d_table_offs, sb_frame_result* d_results, void* scratch, uint64_t scratch_bytes, sb_error* err) {
+    if (!batch || !batch->out_lens || !d_tables || !d_table_offs || !d_results || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K9_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K9_MAX_COUNT);
+    if (batch->count == 0) { ok(err); return -1; }
+    const uint64_t need = frame ? frame_tabled_ws_bytes(batch->count, in_bytes) : raw_tabled_ws_bytes(batch->count, in_bytes);
+    if (need == ~0ull) return fail(err, SB_E_INVALID, batch->count, in_bytes);   // more blocks than one K1 launch takes
+    const uint64_t tb = frame ? sbk::k16_frame_tables_bytes(batch->count, in_bytes)
+                              : sbk::k16_raw_tables_bytes(batch->count, in_bytes);
+    if (tables_bytes < tb) return fail(err, SB_E_INVALID, tables_bytes, tb);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    return 0;
+}
+
+int launch_encode_tabled(Ctx& c, const sb_batch& b, uint64_t in_bytes, bool frame, uint64_t* d_chunk_offs, void* d_tables,
+                         uint64_t* d_table_offs, sb_frame_result* d_results, void* scratch, cudaStream_t st, sb_error* err) {
+    sbk::EncodeTablesPlan t;
+    memset(&t, 0, sizeof t);
+    t.f.r.b = b; t.f.idx = d_chunk_offs;
+    if (frame) sbk::k16_frame_carve(scratch, b.count, in_bytes, &t);
+    else sbk::k16_raw_carve(scratch, b.count, in_bytes, &t);
+    t.tables = (uint8_t*)d_tables; t.table_offs = d_table_offs; t.results = d_results;
+    int rc = frame ? frame_batch_launches(c, t.f, st, err) : raw_compress_launches(c, t.f.r, t.f.crcs, st, err);
+    if (rc) return rc;
+    const unsigned utiles = (unsigned)(((uint64_t)b.count + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    if (frame) k16_size_local_kernel<true><<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(t);
+    else k16_size_local_kernel<false><<<utiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(t);
+    k16_size_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(t);
+    const unsigned eg = device_grid(c, (uint64_t)t.f.r.nslot + b.count + 1, 256, 16);
+    if (frame) k16_frame_export_kernel<<<eg, 256, 0, st>>>(t);
+    else k16_raw_export_kernel<<<eg, 256, 0, st>>>(t);
+    g_launches += 3;
     CK(cudaGetLastError());
     return 0;
 }
@@ -1009,6 +1069,43 @@ int sb_frame_encode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, ui
     int rc = get_ctx(&c, err);
     if (rc) return rc;
     rc = launch_frame_batch(*c, *batch, in_bytes, d_chunk_offs, scratch, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_compress_tables_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k16_raw_tables_bytes(count, in_bytes); }
+uint64_t sb_compress_batch_tabled_scratch_bytes(uint32_t count, uint64_t in_bytes) { return raw_tabled_ws_bytes(count, in_bytes); }
+uint64_t sb_frame_encode_tables_bytes(uint32_t count, uint64_t in_bytes) { return sbk::k16_frame_tables_bytes(count, in_bytes); }
+uint64_t sb_frame_encode_batch_tabled_scratch_bytes(uint32_t count, uint64_t in_bytes) {
+    return frame_tabled_ws_bytes(count, in_bytes);
+}
+
+int sb_compress_batch_tabled_device_ws(const sb_batch* batch, uint64_t in_bytes, void* d_tables, uint64_t tables_bytes,
+                                       uint64_t* d_table_offs, sb_frame_result* d_results, void* scratch,
+                                       uint64_t scratch_bytes, void* stream, sb_error* err) {
+    int rc = tabled_checks(batch, in_bytes, false, d_tables, tables_bytes, d_table_offs, d_results, scratch, scratch_bytes, err);
+    if (rc) return rc < 0 ? 0 : rc;
+    Ctx* c;
+    rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_encode_tabled(*c, *batch, in_bytes, false, nullptr, d_tables, d_table_offs, d_results, scratch,
+                              (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+int sb_frame_encode_batch_tabled_device_ws(const sb_batch* batch, uint64_t in_bytes, uint64_t* d_chunk_offs, void* d_tables,
+                                           uint64_t tables_bytes, uint64_t* d_table_offs, sb_frame_result* d_results,
+                                           void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
+    int rc = tabled_checks(batch, in_bytes, true, d_tables, tables_bytes, d_table_offs, d_results, scratch, scratch_bytes, err);
+    if (rc) return rc < 0 ? 0 : rc;
+    Ctx* c;
+    rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_encode_tabled(*c, *batch, in_bytes, true, d_chunk_offs, d_tables, d_table_offs, d_results, scratch,
+                              (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;

@@ -3,7 +3,7 @@ import ctypes as C
 
 from . import _lib
 from .error import from_c
-from .raw import _ptr
+from .raw import _batch_encode, _ptr, _stored_tables
 
 MAX_BLOCK_SIZE = 1 << 16                      # src/lib.rs:97
 MAX_COMPRESS_BLOCK_SIZE = 76490               # src/frame.rs:12
@@ -33,56 +33,18 @@ def max_len(n: int) -> int:
                                                                                    MAX_COMPRESS_BLOCK_SIZE)
 
 
-def encode_batch(units) -> list:
+def encode_batch(units, tables=False) -> list:
     """Every unit as `FrameEncoder::new(vec![]).write_all(unit); into_inner()`, which is what sb_frame_encode returns: a
     complete framed stream per unit, b"" for an empty one. Units are bytes-like (bytes, bytearray, memoryview, numpy
     arrays). One sb_frame_encode_batch_device_ws call on the current torch stream encodes all of them; the inputs go to
-    the device in one copy and the streams come back in one. Raises the first failing unit's error."""
-    import numpy as np
-    import torch
-    L = _lib.lib()
-    views = [np.frombuffer(u, dtype=np.uint8) for u in units]
-    count = len(views)
-    if count == 0:
-        return []
-    lens = [v.size for v in views]
-    caps = [min(max_len(n), 0xFFFFFFFF) for n in lens]                # a longer unit is BufferTooSmall, never written
-    in_offs = np.zeros(count, dtype=np.int64)
-    in_offs[1:] = np.cumsum(lens[:-1])
-    host = np.empty(sum(lens) + 1, dtype=np.uint8)
-    for o, v in zip(in_offs, views):
-        host[o:o + v.size] = v
-    out_offs = np.zeros(count, dtype=np.int64)
-    room = [c if c == max_len(n) else 0 for n, c in zip(lens, caps)]
-    out_offs[1:] = np.cumsum(room[:-1])
-    # one device buffer holds the streams, then out_lens (u32) and the statuses (sb_error, 32 bytes), 8-byte aligned
-    at_lens = (sum(room) + 7) // 8 * 8
-    at_st = at_lens + (4 * count + 7) // 8 * 8
-    dev = torch.device("cuda", torch.cuda.current_device())
-    t_in = torch.from_numpy(host).to(dev)
-    t_out = torch.empty(at_st + 32 * count, dtype=torch.uint8, device=dev)
-    desc = np.concatenate([in_offs + t_in.data_ptr(), out_offs + t_out.data_ptr(),
-                           np.array(lens + caps, dtype=np.uint32).view(np.int64)])
-    t_desc = torch.from_numpy(desc).to(dev)
-    b = _lib.SbBatch()
-    b.in_ptrs, b.out_ptrs = t_desc.data_ptr(), t_desc.data_ptr() + 8 * count
-    b.in_lens, b.out_caps = t_desc.data_ptr() + 16 * count, t_desc.data_ptr() + 20 * count
-    b.out_lens, b.statuses, b.count = t_out.data_ptr() + at_lens, t_out.data_ptr() + at_st, count
-    in_bytes = sum(n for n, r in zip(lens, room) if n > MAX_BLOCK_SIZE and r)
-    need = L.sb_frame_encode_batch_scratch_bytes(count, in_bytes)
-    t_scr = torch.empty(need, dtype=torch.uint8, device=dev)
-    e = _lib.SbError()
-    if L.sb_frame_encode_batch_device_ws(C.byref(b), in_bytes, None, t_scr.data_ptr(), need,
-                                         torch.cuda.current_stream(dev).cuda_stream, C.byref(e)):
-        raise from_c(e)
-    back = t_out.cpu().numpy()
-    out_lens = back[at_lens:at_lens + 4 * count].view(np.uint32)
-    for st in back[at_st:].view(np.uint64).reshape(count, 4):
-        if st[0] & 0xFFFFFFFF:
-            raise from_c(_lib.SbError(int(st[0] & 0xFFFFFFFF), 0, int(st[1]), int(st[2]), int(st[3])))
-    return [back[o:o + k].tobytes() for o, k in zip(out_offs, out_lens)]
+    the device in one copy and the streams come back in one. Raises the first failing unit's error. tables=True makes
+    the tabled call instead (sb_frame_encode_batch_tabled_device_ws) and returns (streams, tables): every stream's seek
+    table as bytes, what TableReader would build for it, ready to be stored beside it and given to
+    TableReader(..., tables=)."""
+    return _batch_encode(units, lambda n: max_len(n) if max_len(n) <= 0xFFFFFFFF else 0, True, tables)
 
 
+_FRAME_TABLE_MAGIC = 0x0001000042545342    # "BSTB", format version 1 (k13_frame_table.cuh)
 MAX_BATCH_CHUNKS = (1 << 22) - 2             # the largest chunk table sb_frame_decode_batch_device_ws takes
 
 
@@ -296,12 +258,16 @@ class TableReader:
     then serves ranges of any of the streams in one library call per group, decoding and checksumming only the chunks
     they cover, with no pass over any stream's headers. Every range gives what `RangeReader(streams[i]).read(lo, n)`
     gives. A stream is a bytes-like object (uploaded once) or a contiguous 1-D CUDA uint8 tensor (kept alive).
-    fragment: the streams have no identifier. Calls run on the current torch stream and wait for their results."""
+    fragment: the streams have no identifier. Calls run on the current torch stream and wait for their results.
+    tables: the streams' stored seek tables (from encode_batch(..., tables=True) or an earlier build), bytes-like or
+    CUDA uint8 tensors, instead of a build. They are uploaded in one copy and no build runs; a table whose header does
+    not match its stream's length raises ValueError. A table of another stream of the same length gives the reads over
+    it a chunk's checksum error, never wrong bytes."""
 
     RANGES_PER_CALL = RangeReader.RANGES_PER_CALL
     BYTES_PER_CALL = RangeReader.BYTES_PER_CALL
 
-    def __init__(self, streams, fragment=False):
+    def __init__(self, streams, fragment=False, tables=None):
         import numpy as np
         import torch
         self._dev = torch.device("cuda", torch.cuda.current_device())
@@ -327,6 +293,12 @@ class TableReader:
         count = len(self._ins)
         lens = [t.numel() for t in self._ins]
         self._bufs = []                                                  # the tables live in these
+        if tables is not None:
+            self._bufs, heads = _stored_tables(tables, lens, self._dev, _FRAME_TABLE_MAGIC, 32,
+                                               lambda w: int(w[3]) & 0xFFFFFFFF)
+            self.lengths = [int(w[2]) for w in heads]
+            self._keep_tables([t.data_ptr() for t in self._bufs], lens)
+            return
         ptrs, results = [0] * count, [None] * count
         # a stream that fits an sb_batch unit is tabled in a batch call; a longer one gets a build of its own
         for i, t, r in zip(*self._build([i for i in range(count) if lens[i] > 0xFFFFFFFF], flags)):
@@ -340,6 +312,12 @@ class TableReader:
                 ptrs[i], results[i] = p, r
             todo = [i for i in todo if results[i].status.code == 202 and results[i].status.b == 1]
         self.lengths = [int(r.bytes) for r in results]
+        self._keep_tables(ptrs, lens)
+
+    def _keep_tables(self, ptrs, lens):
+        """The device arrays of table addresses, stream addresses and stream lengths every read passes."""
+        import numpy as np
+        import torch
         to64 = lambda v: torch.from_numpy(np.array(v, dtype=np.uint64).view(np.int64)).to(self._dev)
         self._t_tables = to64(ptrs + [0])
         self._t_ins = to64([t.data_ptr() for t in self._ins] + [0])

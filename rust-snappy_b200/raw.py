@@ -78,6 +78,131 @@ def crc32c_masked(data) -> int:
     return out.value
 
 
+_RAW_TABLE_MAGIC = 0x0001000042545352      # "RSTB", format version 1 (k15_raw_table.cuh)
+
+
+def _batch_encode(units, cap_of, frame, tables):
+    """One sb_compress_batch_device_ws (frame: sb_frame_encode_batch_device_ws) call over bytes-like units, or its tabled
+    form: the inputs go to the device in one copy, the streams (and tables) come back in one. cap_of(n) is the unit's
+    cap, 0 for a unit the call rejects without writing. Raises the first failing unit's error."""
+    import numpy as np
+    import torch
+    L = _lib.lib()
+    views = [np.frombuffer(u, dtype=np.uint8) for u in units]
+    count = len(views)
+    if count == 0:
+        return ([], []) if tables else []
+    lens = [v.size for v in views]
+    caps = [cap_of(n) for n in lens]
+    in_offs = np.zeros(count, dtype=np.int64)
+    in_offs[1:] = np.cumsum(lens[:-1])
+    host = np.empty(sum(lens) + 1, dtype=np.uint8)
+    for o, v in zip(in_offs, views):
+        host[o:o + v.size] = v
+    out_offs = np.zeros(count, dtype=np.int64)
+    out_offs[1:] = np.cumsum(caps[:-1])
+    # one device buffer holds the streams, then out_lens (u32) and the statuses (sb_error, 32 bytes), 8-byte aligned
+    at_lens = (sum(caps) + 7) // 8 * 8
+    at_st = at_lens + (4 * count + 7) // 8 * 8
+    dev = torch.device("cuda", torch.cuda.current_device())
+    t_in = torch.from_numpy(host).to(dev)
+    t_out = torch.empty(at_st + 32 * count, dtype=torch.uint8, device=dev)
+    desc = np.concatenate([in_offs + t_in.data_ptr(), out_offs + t_out.data_ptr(),
+                           np.array(lens + [c if c else 0xFFFFFFFF * frame for c in caps], dtype=np.uint32).view(np.int64)])
+    t_desc = torch.from_numpy(desc).to(dev)
+    b = _lib.SbBatch()
+    b.in_ptrs, b.out_ptrs = t_desc.data_ptr(), t_desc.data_ptr() + 8 * count
+    b.in_lens, b.out_caps = t_desc.data_ptr() + 16 * count, t_desc.data_ptr() + 20 * count
+    b.out_lens, b.statuses, b.count = t_out.data_ptr() + at_lens, t_out.data_ptr() + at_st, count
+    in_bytes = sum(n for n, c in zip(lens, caps) if n > 65536 and c)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    e = _lib.SbError()
+    if tables:
+        tb = (L.sb_frame_encode_tables_bytes if frame else L.sb_compress_tables_bytes)(count, in_bytes)
+        need = (L.sb_frame_encode_batch_tabled_scratch_bytes if frame else L.sb_compress_batch_tabled_scratch_bytes)(
+            count, in_bytes)
+        t_scr = torch.empty(need, dtype=torch.uint8, device=dev)
+        t_tab = torch.empty(tb + 8 * (count + 1) + C.sizeof(_lib.SbFrameResult) * count, dtype=torch.uint8, device=dev)
+        p = t_tab.data_ptr()
+        args = (p, tb, p + tb, p + tb + 8 * (count + 1), t_scr.data_ptr(), need, stream, C.byref(e))
+        rc = L.sb_frame_encode_batch_tabled_device_ws(C.byref(b), in_bytes, None, *args) if frame else \
+            L.sb_compress_batch_tabled_device_ws(C.byref(b), in_bytes, *args)
+    else:
+        need = (L.sb_frame_encode_batch_scratch_bytes if frame else L.sb_compress_batch_scratch_bytes)(count, in_bytes)
+        t_scr = torch.empty(need, dtype=torch.uint8, device=dev)
+        rc = L.sb_frame_encode_batch_device_ws(C.byref(b), in_bytes, None, t_scr.data_ptr(), need, stream, C.byref(e)) \
+            if frame else L.sb_compress_batch_device_ws(C.byref(b), in_bytes, t_scr.data_ptr(), need, stream, C.byref(e))
+    if rc:
+        raise from_c(e)
+    back = t_out.cpu().numpy()
+    out_lens = back[at_lens:at_lens + 4 * count].view(np.uint32)
+    for st in back[at_st:].view(np.uint64).reshape(count, 4):
+        if st[0] & 0xFFFFFFFF:
+            raise from_c(_lib.SbError(int(st[0] & 0xFFFFFFFF), 0, int(st[1]), int(st[2]), int(st[3])))
+    streams = [back[o:o + k].tobytes() for o, k in zip(out_offs, out_lens)]
+    if not tables:
+        return streams
+    offs = t_tab[tb:tb + 8 * (count + 1)].cpu().numpy().view(np.uint64)
+    packed = t_tab[:int(offs[count])].cpu().numpy()
+    return streams, [packed[int(offs[i]):int(offs[i + 1])].tobytes() for i in range(count)]
+
+
+def compress_batch(units, tables=False):
+    """Every unit as `Encoder().compress_vec(unit)` returns it, in one sb_compress_batch_device_ws call on the current
+    torch stream. Units are bytes-like (bytes, bytearray, memoryview, numpy arrays); the inputs go to the device in one
+    copy and the streams come back in one. Raises the first failing unit's error. tables=True makes the tabled call
+    instead (sb_compress_batch_tabled_device_ws) and returns (streams, tables): every stream's raw seek table as
+    bytes, what TableReader would build for it, ready to be stored beside it and given to TableReader(..., tables=)."""
+    return _batch_encode(units, lambda n: max_compress_len(n) if n < 0xFFFFFFFF else 0, False, tables)
+
+
+def _stored_tables(tables, lens, dev, magic, rec, records):
+    """Tables given to a reader: bytes-like ones go to the device in one copy, CUDA uint8 tensors are kept. Every header
+    is checked on the host (size, magic, the stream length it was built over); records(words) is the record count a
+    header announces. Returns (device tensors, headers as arrays of eight 64-bit words)."""
+    import numpy as np
+    import torch
+    tables = list(tables)
+    if len(tables) != len(lens):
+        raise ValueError("%d tables for %d streams" % (len(tables), len(lens)))
+    out, host = [], []
+    for i, t in enumerate(tables):
+        if isinstance(t, torch.Tensor):
+            if not t.is_cuda or t.dtype != torch.uint8 or t.dim() != 1 or not t.is_contiguous() or t.data_ptr() % 8:
+                raise ValueError("table %d: tables are bytes-like or contiguous 1-D 8-byte aligned CUDA uint8 tensors" % i)
+            out.append(t)
+        else:
+            v = np.frombuffer(t, dtype=np.uint8)
+            host.append((i, v))
+            out.append(None)
+    if host:                                                             # 8-byte multiples, so every table stays aligned
+        at = np.cumsum([0] + [(v.size + 7) // 8 * 8 for _, v in host])
+        cat = np.zeros(int(at[-1]) + 8, dtype=np.uint8)
+        for (_, v), o in zip(host, at):
+            cat[o:o + v.size] = v
+        t_all = torch.from_numpy(cat).to(dev)
+        for (i, v), o in zip(host, at):
+            out[i] = t_all[int(o):int(o) + v.size]
+    heads = {i: v[:64] for i, v in host if v.size >= 64}
+    dev_heads = [i for i, t in enumerate(out) if i not in heads and t.numel() >= 64]
+    if dev_heads:
+        back = torch.stack([out[i][:64] for i in dev_heads]).cpu().numpy()
+        heads.update(zip(dev_heads, back))
+    words = []
+    for i, (t, n) in enumerate(zip(out, lens)):
+        if i not in heads:
+            raise ValueError("table %d has %d bytes; a table has a 64-byte header" % (i, t.numel()))
+        w = np.frombuffer(np.ascontiguousarray(heads[i]).tobytes(), dtype=np.uint64)
+        if int(w[0]) != magic:
+            raise ValueError("table %d is not a seek table of this format" % i)
+        if int(w[1]) != n:
+            raise ValueError("table %d was built over a stream of %d bytes; stream %d has %d" % (i, int(w[1]), i, n))
+        if t.numel() < 64 + rec * records(w):
+            raise ValueError("table %d has %d bytes; its header announces %d records" % (i, t.numel(), records(w)))
+        words.append(w)
+    return out, words
+
+
 class TableReader:
     """Random access to the decoded bytes of many raw streams on the device. Each stream gets a seek table, built once on
     the device in batch calls (sb_raw_table_build_batch_device_ws), one per group of streams whatever their number: the
@@ -87,13 +212,17 @@ class TableReader:
     seekable (see `seekable`: not block-independent, or not decodable) is decoded whole on the device for each call
     that reads it, and gives exactly that slice or raises that call's error. A stream is a bytes-like object (uploaded
     with the others in one copy) or a contiguous 1-D CUDA uint8 tensor (kept alive), of at most 2^32 - 1 bytes. Calls run
-    on the current torch stream and wait for their results."""
+    on the current torch stream and wait for their results.
+    tables: the streams' stored seek tables (from compress_batch(..., tables=True) or an earlier build), bytes-like or
+    CUDA uint8 tensors, instead of a build. They are uploaded in one copy and no build runs; a table whose header does
+    not match its stream's length raises ValueError. A table of another stream of the same length gives every read over
+    it that block's checksum error, never wrong bytes."""
 
     RANGES_PER_CALL = 4096                    # 128 KiB of staging per range: 512 MiB per call at most
     BYTES_PER_CALL = 1 << 30                  # output bytes one call gathers (a single larger range gets its own call)
     GROUP_BYTES = 1 << 34                     # compressed bytes one build call takes (its scratch grows with them)
 
-    def __init__(self, streams):
+    def __init__(self, streams, tables=None):
         import numpy as np
         import torch
         self._dev = torch.device("cuda", torch.cuda.current_device())
@@ -124,11 +253,18 @@ class TableReader:
                 raise ValueError("stream %d has %d bytes; a raw stream has at most 2^32 - 1" % (i, n))
         count = len(self._ins)
         self._bufs = []                                                  # the tables live in these
-        ptrs, results = [0] * count, [None] * count
-        for i, p, r in self._build(list(range(count))):
-            ptrs[i], results[i] = p, r
-        self.seekable = [r.status.code == 0 for r in results]
-        self.lengths = [int(r.bytes) if ok else None for r, ok in zip(results, self.seekable)]
+        if tables is not None:
+            self._bufs, heads = _stored_tables(tables, lens, self._dev, _RAW_TABLE_MAGIC, 8,
+                                               lambda w: int(w[3]) >> 32)
+            ptrs = [t.data_ptr() for t in self._bufs]
+            self.seekable = [int(w[4]) & 0xFFFFFFFF == 1 for w in heads]
+            self.lengths = [int(w[2]) if ok else None for w, ok in zip(heads, self.seekable)]
+        else:
+            ptrs, results = [0] * count, [None] * count
+            for i, p, r in self._build(list(range(count))):
+                ptrs[i], results[i] = p, r
+            self.seekable = [r.status.code == 0 for r in results]
+            self.lengths = [int(r.bytes) if ok else None for r, ok in zip(results, self.seekable)]
         to64 = lambda v: torch.from_numpy(np.array(v, dtype=np.uint64).view(np.int64)).to(self._dev)
         self._t_tables = to64(ptrs + [0])
         self._t_ins = to64([t.data_ptr() for t in self._ins] + [0])
