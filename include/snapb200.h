@@ -464,6 +464,34 @@ int sb_raw_table_decode_ranges_device_ws(const void* const* d_tables, const uint
                                          uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
                                          uint64_t scratch_bytes, void* stream, sb_error* err);
 
+/* Gathers: many small ranges over tabled frame or raw streams in one call. The arguments are exactly those of
+ * sb_frame_table_decode_ranges_device_ws / sb_raw_table_decode_ranges_device_ws, and so is the result: every range gets
+ * the status, out_len and bytes [out_r, out_r + out_len) that call gives it, and nothing outside
+ * [out_r, out_r + max(end - lo, 0)) is written. No table content makes the call read outside a stream or write outside
+ * a range's buffer or the scratch. What differs is the cost:
+ *   - an interior chunk or block (inside [lo, end) in full) decodes straight into its range's buffer, once per range
+ *     that holds it, as in the range calls;
+ *   - an edge chunk or block (the head or tail one, straddling lo or end) is decoded and CRC-checked once per call,
+ *     however many ranges share it as an edge. A chunk that is an edge of more than 256 ranges is decoded once per group
+ *     of at most 256 of them, so that one hot key does not serialise a call behind one warp;
+ *   - a chunk that is interior to one range and an edge of another is decoded once in each role.
+ * The scratch, sb_*_gather_scratch_bytes(nranges), is 108 bytes per range of bookkeeping (a hash table of the edges and
+ * their per-chunk lists), a few KiB of scan tiles and alignment, and a staging pool of min(2 * nranges, 4096) slots of
+ * 64 KiB, one per decoding warp: at most 128 * nranges + 256 MiB + 64 KiB bytes whatever nranges, and within 3 KiB of the
+ * range calls' scratch for one range. Stream ordered, no allocation, no host synchronisation, and the same launches
+ * whatever count, nranges and the sharing pattern; nranges == 0 does nothing. Null pointers that are needed,
+ * count >= 2^31, nranges > 2^28 and scratch that is too small are SB_E_INVALID with nothing launched. */
+uint64_t sb_frame_table_gather_scratch_bytes(uint32_t nranges);
+int sb_frame_table_gather_device_ws(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens,
+                                    uint32_t count, const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len,
+                                    uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
+                                    uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
+uint64_t sb_raw_table_gather_scratch_bytes(uint32_t nranges);
+int sb_raw_table_gather_device_ws(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens,
+                                  uint32_t count, const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len,
+                                  uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
+                                  uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
+
 /* Batch encoders that also write one seek table per unit, so what they write is seekable without a build. Each does
  * exactly what its untabled call does: output bytes, out_lens, statuses and (frame) d_chunk_offs are byte-identical to
  * sb_compress_batch_device_ws / sb_frame_encode_batch_device_ws with the same arguments, rejected units and the in_bytes

@@ -46,6 +46,8 @@ SYMBOLS = [
     "sb_frame_table_batch_bytes", "sb_frame_table_build_batch_scratch_bytes", "sb_frame_table_build_batch_device_ws",
     "sb_raw_table_bytes", "sb_raw_table_batch_bytes", "sb_raw_table_build_batch_scratch_bytes",
     "sb_raw_table_build_batch_device_ws", "sb_raw_table_ranges_scratch_bytes", "sb_raw_table_decode_ranges_device_ws",
+    "sb_frame_table_gather_scratch_bytes", "sb_frame_table_gather_device_ws", "sb_raw_table_gather_scratch_bytes",
+    "sb_raw_table_gather_device_ws",
     "sb_compress_tables_bytes", "sb_compress_batch_tabled_scratch_bytes", "sb_compress_batch_tabled_device_ws",
     "sb_frame_encode_tables_bytes", "sb_frame_encode_batch_tabled_scratch_bytes", "sb_frame_encode_batch_tabled_device_ws",
     "sb_frame_max_len", "sb_frame_encode", "sb_frame_encode_ex", "sb_frame_decode", "sb_frame_encode_device",
@@ -133,6 +135,11 @@ def lib():
     L.sb_raw_table_ranges_scratch_bytes.argtypes = [C.c_uint32]
     L.sb_raw_table_decode_ranges_device_ws.argtypes = [vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp, C.c_uint32, vp,
                                                        C.c_uint64, vp, ep]
+    for fmt in ("frame", "raw"):
+        getattr(L, "sb_%s_table_gather_scratch_bytes" % fmt).restype = C.c_uint64
+        getattr(L, "sb_%s_table_gather_scratch_bytes" % fmt).argtypes = [C.c_uint32]
+        getattr(L, "sb_%s_table_gather_device_ws" % fmt).argtypes = [vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp,
+                                                                     C.c_uint32, vp, C.c_uint64, vp, ep]
     for name in ("sb_compress_tables_bytes", "sb_compress_batch_tabled_scratch_bytes", "sb_frame_encode_tables_bytes",
                  "sb_frame_encode_batch_tabled_scratch_bytes"):
         getattr(L, name).restype = C.c_uint64

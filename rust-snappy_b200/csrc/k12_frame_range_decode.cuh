@@ -27,7 +27,7 @@
 // A table that is too small leaves total a lower bound, so every range reports it first, as k5_finish does.
 //
 // Costs. A chunk shared by several ranges is decoded once per range, and each range takes 128 KiB of staging whatever
-// its length; callers with very many small ranges split them over several calls.
+// its length; callers with very many small ranges over tabled streams use the gathers (k17_table_gather.cuh).
 #pragma once
 #include "k5_frame_decode.cuh"
 #include "k8_raw_split.cuh"
@@ -68,6 +68,31 @@ inline uint64_t k12_carve(void* scratch, uint32_t nranges, RangePlan* q) {
     if (q) { q->nranges = nranges; q->rec = rec; q->pr_offs = offs; q->pr_tiles = tiles; q->staging = staging; }
     return at + 256;
 }
+
+// The gather calls (k17_table_gather.cuh) replace the two staging slots per range by a pool of k17_pool_slots(nranges)
+// slots of K12_SLOT bytes, one per warp that decodes into staging: the gather decode and K13's finish body run only the
+// first k12_pool_warps warps of their grid, warp w on slot w. The one definition of the pool's size, for the carve, the
+// launch grids and the bodies.
+static const uint32_t K17_SLOTS = 4096;
+#if defined(SB_EMU)
+static inline uint64_t k17_pool_slots(uint32_t nranges)
+#else
+__host__ __device__ __forceinline__ uint64_t k17_pool_slots(uint32_t nranges)
+#endif
+{
+    return 2ull * nranges < K17_SLOTS ? 2ull * nranges : K17_SLOTS;
+}
+SB_DEVICE uint64_t k12_pool_warps(uint64_t nwarps, uint32_t nranges) {
+    const uint64_t slots = k17_pool_slots(nranges);
+    return nwarps < slots ? nwarps : slots;
+}
+// Emulator builds count the chunk and block decodes of the gather calls, so the tests can check their cost contract
+#if defined(SB_EMU)
+inline uint64_t g_emu_decodes = 0;
+#define K17_COUNT_DECODE() do { if (lane_id() == 0) sbk::g_emu_decodes++; } while (0)
+#else
+#define K17_COUNT_DECODE() do {} while (0)
+#endif
 
 SB_DEVICE bool k12_table_full(const DecodeCtl* c) { return c->walk_err.code == SB_E_INVALID && c->walk_err.b == 1; }
 // min(lo + len, total) without overflow

@@ -148,6 +148,10 @@ SB_DEVICE void k13_plan_body(const TablePlan& q) {
 }
 SB_DEVICE void k13_plan_tiles_body(const TablePlan& q) { scan_tiles_body(q.nranges + 1, 0, q.pr_tiles); }
 
+// GATHER (the gather call, k17_table_gather.cuh): only pairs inside [lo, end) decode here, on the whole grid. The head
+// and tail pairs that are not inside are left to K17's gather decode. A middle pair that is not inside (only a table
+// whose offsets were tampered with has one) sets rec[r]._pad, and the gather's finish walks that range's run for it.
+template <bool GATHER = false>
 SB_DEVICE void k13_decode_body(const TablePlan& q) {
     uint32_t* tab = (uint32_t*)smem();                                // K3 slicing tables (4 KB)
     k3_build_tables(tab);
@@ -166,7 +170,13 @@ SB_DEVICE void k13_decode_body(const TablePlan& q) {
         uint32_t code = SB_E_INVALID;
         if (k13_rec_ok(t, h->n, lo, end)) {
             const bool inside = t.off >= lo && t.off + t.dlen <= end;
+            if (GATHER && !inside) {
+                if (k != first && k + 1 != first + q.rec[r].pairs && lane_id() == 0) q.rec[r]._pad = 1;
+                syncwarp();
+                continue;
+            }
             uint8_t* dst = inside ? q.outs[r] + (t.off - lo) : q.staging + ((uint64_t)r * 2 + (k == first ? 0 : 1)) * K12_SLOT;
+            if (GATHER) K17_COUNT_DECODE();
             code = k5_decode_chunk(tab, elems, k13_chunk(t), q.ins[u], dst, sink);
             if (code == SB_OK && !inside) {                               // the slice of [lo, end) a head or tail chunk holds
                 const uint64_t a = t.off > lo ? t.off : lo, e = t.off + t.dlen < end ? t.off + t.dlen : end;
@@ -179,15 +189,20 @@ SB_DEVICE void k13_decode_body(const TablePlan& q) {
 }
 
 // per range, in priority order: unit out of range, not a table of this stream, chunk table too small, the first failing
-// verified chunk, past the end: the walk's stopping error (Ok at a clean end), else Ok
+// verified chunk, past the end: the walk's stopping error (Ok at a clean end), else Ok. GATHER: a range whose rec._pad the
+// interior decode set first decodes its middle pairs that are not inside [lo, end) into the warp's pool slot, as the
+// range call decodes them into its staging; the failing chunk decodes again into that slot.
+template <bool GATHER = false>
 SB_DEVICE void k13_finish_body(const TablePlan& q) {
     uint32_t* tab = (uint32_t*)smem();
     k3_build_tables(tab);
     uint32_t* elems = (uint32_t*)(smem() + K3_TABLE_BYTES) + warp_id() * 64;
     const unsigned wpb = block_dim() >> 5;
     const bool lead = lane_id() == 0;
-    const uint64_t nwarps = (uint64_t)grid_dim() * wpb;
-    for (uint64_t r = (uint64_t)block_idx() * wpb + warp_id(); r < q.nranges; r += nwarps) {
+    uint64_t nwarps = (uint64_t)grid_dim() * wpb;
+    const uint64_t w = (uint64_t)block_idx() * wpb + warp_id();
+    if (GATHER) { nwarps = k12_pool_warps(nwarps, q.nranges); if (w >= nwarps) return; }
+    for (uint64_t r = w; r < q.nranges; r += nwarps) {
         const uint32_t u = q.unit[r];
         const TableHead* h = k13_head(q, (uint32_t)r);
         sb_error* st = &q.statuses[r];
@@ -202,13 +217,29 @@ SB_DEVICE void k13_finish_body(const TablePlan& q) {
             }
         } else {
             const uint64_t total = h->total, lo = q.lo[r], len = q.len[r], end = k12_end(lo, len, total);
+            if (GATHER && q.rec[r]._pad) {
+                const RangeRec rr = q.rec[r];
+                uint8_t* slot = q.staging + w * K12_SLOT;
+                for (uint32_t k = rr.first + 1; k + 1 < rr.first + rr.pairs; k++) {
+                    const TableRec t = k13_recs(h)[k];
+                    if (!k13_rec_ok(t, h->n, lo, end) || (t.off >= lo && t.off + t.dlen <= end)) continue;
+                    // st takes the chunk's status for now; every branch below writes the range's own
+                    if (k5_decode_chunk(tab, elems, k13_chunk(t), q.ins[u], slot, st) != SB_OK) {
+                        if (lead) atomic_min(&q.rec[r].first_bad, k);
+                    } else {
+                        const uint64_t a = t.off > lo ? t.off : lo, e = t.off + t.dlen < end ? t.off + t.dlen : end;
+                        warp_copy(q.outs[r] + (a - lo), slot + (a - t.off), (uint32_t)(e - a));
+                    }
+                    syncwarp();
+                }
+            }
             const uint32_t bad = q.rec[r].first_bad;
             got = end > lo ? end - lo : 0;
             if (h->full) { if (lead) *st = h->walk_err; got = 0; }
             else if (bad != K12_NONE) {
                 const TableRec t = k13_recs(h)[bad];
                 if (!k13_rec_ok(t, h->n, lo, end)) { if (lead) set_status(st, SB_E_INVALID, bad, 0, 3); }
-                else k5_decode_chunk(tab, elems, k13_chunk(t), q.ins[u], q.staging + r * 2 * K12_SLOT, st);
+                else k5_decode_chunk(tab, elems, k13_chunk(t), q.ins[u], q.staging + (GATHER ? w : r * 2) * K12_SLOT, st);
                 const uint64_t stop = t.off < end ? t.off : end;           // off_k* for a valid table
                 got = stop > lo ? stop - lo : 0;
             }

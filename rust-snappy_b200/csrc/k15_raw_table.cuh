@@ -293,6 +293,10 @@ SB_DEVICE void k15_plan_body(const RawRangePlan& q) {
 }
 SB_DEVICE void k15_plan_tiles_body(const RawRangePlan& q) { scan_tiles_body(q.nranges + 1, 0, q.pr_tiles); }
 
+// GATHER (the gather call, k17_table_gather.cuh): the head and tail pairs that are not inside [lo, end) are left to K17's
+// gather decode (only they can straddle lo or end: blocks are implied by their index), so no warp needs staging and
+// the whole grid decodes.
+template <bool GATHER = false>
 SB_DEVICE void k15_decode_body(const RawRangePlan& q) {
     uint32_t* tab = (uint32_t*)smem();                                // K3 slicing tables (4 KB)
     k3_build_tables(tab);
@@ -312,7 +316,9 @@ SB_DEVICE void k15_decode_body(const RawRangePlan& q) {
             const uint64_t dl = h->dn - off < 65536 ? h->dn - off : 65536;
             const uint32_t a = t[j].off, b = j + 1 < h->nblocks ? t[j + 1].off : (uint32_t)h->n;
             const bool inside = off >= lo && off + dl <= end;
+            if (GATHER && !inside) { syncwarp(); continue; }
             uint8_t* dst = inside ? q.outs[r] + (off - lo) : q.staging + ((uint64_t)r * 2 + (j == first ? 0 : 1)) * K12_SLOT;
+            if (GATHER) K17_COUNT_DECODE();
             code = k2_decode_stream<false>(q.ins[u] + a, b - a, dst, dl, nullptr, nullptr, elems);
             syncwarp();
             if (code == SB_OK && k3_warp_crc32c_masked(tab, dst, (uint32_t)dl) != t[j].crc) code = SB_CHECKSUM;

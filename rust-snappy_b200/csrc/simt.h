@@ -17,6 +17,12 @@
 namespace sbk {
 // the emulator has no caches: a prefetch is a hint with nothing to do
 SB_DEVICE void prefetch_l2(const void*) {}
+// fibers switch only at warp collectives, so a plain compare-and-swap is atomic
+SB_DEVICE unsigned long long atomic_cas(unsigned long long* p, unsigned long long cmp, unsigned long long v) {
+    const unsigned long long o = *p;
+    if (o == cmp) *p = v;
+    return o;
+}
 }
 #else
 
@@ -66,6 +72,9 @@ SB_DEVICE uint32_t byte_perm(uint32_t a, uint32_t b, uint32_t s) { return __byte
 SB_DEVICE uint32_t atomic_add(uint32_t* p, uint32_t v) { return atomicAdd(p, v); }
 SB_DEVICE unsigned long long atomic_add(unsigned long long* p, unsigned long long v) { return atomicAdd(p, v); }
 SB_DEVICE uint32_t atomic_min(uint32_t* p, uint32_t v) { return atomicMin(p, v); }
+SB_DEVICE unsigned long long atomic_cas(unsigned long long* p, unsigned long long cmp, unsigned long long v) {
+    return atomicCAS(p, cmp, v);
+}
 SB_DEVICE void threadfence() { __threadfence(); }
 SB_DEVICE void threadfence_block() { __threadfence_block(); }
 SB_DEVICE uint32_t reduce_or(uint32_t v) { return __reduce_or_sync(SB_FULL, v); }

@@ -29,6 +29,7 @@
 #include "k14_frame_table_batch.cuh"
 #include "k15_raw_table.cuh"
 #include "k16_encode_tables.cuh"
+#include "k17_table_gather.cuh"
 
 namespace {
 
@@ -139,6 +140,24 @@ __global__ void __launch_bounds__(1024) k16_size_local_kernel(sbk::EncodeTablesP
 __global__ void __launch_bounds__(1024) k16_size_tiles_kernel(sbk::EncodeTablesPlan t) { sbk::k16_size_tiles_body(t); }
 __global__ void __launch_bounds__(256) k16_raw_export_kernel(sbk::EncodeTablesPlan t) { sbk::k16_raw_export_body(t); }
 __global__ void __launch_bounds__(256) k16_frame_export_kernel(sbk::EncodeTablesPlan t) { sbk::k16_frame_export_body(t); }
+
+template <class P>
+__global__ void __launch_bounds__(256) k17_clear_kernel(sbk::GatherPlan<P> g) { sbk::k17_clear_body(g); }
+template <class P>
+__global__ void __launch_bounds__(256) k17_insert_kernel(sbk::GatherPlan<P> g) { sbk::k17_insert_body(g); }
+template <class P>
+__global__ void __launch_bounds__(1024) k17_scan_local_kernel(sbk::GatherPlan<P> g) { sbk::k17_scan_local_body(g); }
+template <class P>
+__global__ void __launch_bounds__(1024) k17_scan_tiles_kernel(sbk::GatherPlan<P> g) { sbk::k17_scan_tiles_body(g); }
+template <class P>
+__global__ void __launch_bounds__(256) k17_fill_kernel(sbk::GatherPlan<P> g) { sbk::k17_fill_body(g); }
+// the interior decodes: K13's and K15's decode budget and grid, every warp decoding; the gather decodes keep 8 CTAs of
+// 128 per SM, so that the pool's 4,096 warps all run
+__global__ void __launch_bounds__(128, 4) k17_frame_interior_kernel(sbk::TablePlan q) { sbk::k13_decode_body<true>(q); }
+__global__ void __launch_bounds__(128, 4) k17_raw_interior_kernel(sbk::RawRangePlan q) { sbk::k15_decode_body<true>(q); }
+__global__ void __launch_bounds__(128, 8) k17_frame_gather_kernel(sbk::GatherPlan<sbk::TablePlan> g) { sbk::k17_frame_gather_body(g); }
+__global__ void __launch_bounds__(128, 8) k17_raw_gather_kernel(sbk::GatherPlan<sbk::RawRangePlan> g) { sbk::k17_raw_gather_body(g); }
+__global__ void __launch_bounds__(128) k17_frame_finish_kernel(sbk::TablePlan q) { sbk::k13_finish_body<true>(q); }
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -912,6 +931,85 @@ int launch_raw_table_ranges(Ctx& c, const sbk::RawRangePlan& q, cudaStream_t st,
     return 0;
 }
 
+
+// ---- gathers over tabled frame and raw streams (K17): the range plan, the edge lists, the interior decode, the gather
+// decode over the pool, the finish. 10 launches.
+template <class P>
+int launch_gather_lists(Ctx& c, const sbk::GatherPlan<P>& g, cudaStream_t st, sb_error* err) {
+    const unsigned stiles = (unsigned)(((uint64_t)g.nh + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    k17_clear_kernel<P><<<device_grid(c, g.nh, 256, 16), 256, 0, st>>>(g);
+    k17_insert_kernel<P><<<device_grid(c, g.q.nranges, 256, 16), 256, 0, st>>>(g);
+    k17_scan_local_kernel<P><<<stiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(g);
+    k17_scan_tiles_kernel<P><<<1, 1024, 1024 * sizeof(uint64_t), st>>>(g);
+    k17_fill_kernel<P><<<device_grid(c, g.q.nranges, 256, 16), 256, 0, st>>>(g);
+    g_launches += 5;
+    CK(cudaGetLastError());
+    return 0;
+}
+int launch_frame_table_gather(Ctx& c, const sbk::GatherPlan<sbk::TablePlan>& g, cudaStream_t st, sb_error* err) {
+    const sbk::TablePlan& q = g.q;
+    const uint64_t most = (uint64_t)16 * c.sms, fw = ((uint64_t)q.nranges + 3) / 4, slots = sbk::k17_pool_slots(q.nranges);
+    const unsigned ptiles = (unsigned)(((uint64_t)q.nranges + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    const uint32_t smem = sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP;
+    k13_plan_kernel<<<ptiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k13_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    g_launches += 2;
+    int rc = launch_gather_lists(c, g, st, err);
+    if (rc) return rc;
+    k17_frame_interior_kernel<<<(unsigned)most, 128, smem + 4 * sizeof(sb_error), st>>>(q);
+    k17_frame_gather_kernel<<<(unsigned)((slots + 3) / 4), 128, smem + 4 * sizeof(sb_error), st>>>(g);
+    k17_frame_finish_kernel<<<fw < most ? (unsigned)fw : (unsigned)most, 128, smem, st>>>(q);
+    g_launches += 3;
+    CK(cudaGetLastError());
+    return 0;
+}
+int launch_raw_table_gather(Ctx& c, const sbk::GatherPlan<sbk::RawRangePlan>& g, cudaStream_t st, sb_error* err) {
+    const sbk::RawRangePlan& q = g.q;
+    const unsigned ptiles = (unsigned)(((uint64_t)q.nranges + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
+    const uint64_t slots = sbk::k17_pool_slots(q.nranges);
+    const uint32_t smem = sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP;
+    k15_plan_kernel<<<ptiles, sbk::K4_TILE, 32 * sizeof(uint32_t), st>>>(q);
+    k15_plan_tiles_kernel<<<1, 1024, 1024 * sizeof(uint64_t), st>>>(q);
+    g_launches += 2;
+    int rc = launch_gather_lists(c, g, st, err);
+    if (rc) return rc;
+    k17_raw_interior_kernel<<<16 * c.sms, 128, smem, st>>>(q);
+    k17_raw_gather_kernel<<<(unsigned)((slots + 3) / 4), 128, smem, st>>>(g);
+    k15_finish_kernel<<<device_grid(c, q.nranges, 256, 16), 256, 0, st>>>(q);
+    g_launches += 3;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// the call checks of the range calls, with the gathers' range limit and scratch
+template <class P>
+int gather_call(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens, uint32_t count,
+                const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch, uint64_t scratch_bytes,
+                void* stream, sb_error* err,
+                int (*launch)(Ctx&, const sbk::GatherPlan<P>&, cudaStream_t, sb_error*)) {
+    if (count >= sbk::K13_MAX_COUNT) return fail(err, SB_E_INVALID, count, sbk::K13_MAX_COUNT);
+    if (nranges > sbk::K17_MAX_RANGES) return fail(err, SB_E_INVALID, nranges, sbk::K17_MAX_RANGES);
+    if (nranges == 0) { ok(err); return 0; }
+    if (count && (!d_tables || !d_ins || !d_in_lens)) return fail(err, SB_E_INVALID);
+    if (!d_unit || !d_lo || !d_len || !d_out_ptrs || !d_out_lens || !d_statuses || !scratch) return fail(err, SB_E_INVALID);
+    const uint64_t need = sbk::k17_carve<P>(nullptr, nranges, nullptr);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    sbk::GatherPlan<P> g;
+    memset(&g, 0, sizeof g);
+    P& q = g.q;
+    q.tables = d_tables; q.ins = d_ins; q.in_lens = d_in_lens; q.count = count;
+    q.unit = d_unit; q.lo = d_lo; q.len = d_len; q.outs = d_out_ptrs; q.out_lens = d_out_lens; q.statuses = d_statuses;
+    sbk::k17_carve(scratch, nranges, &g);
+    rc = launch(*c, g, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
 }  // namespace
 
 // =========================================================================
@@ -1289,6 +1387,27 @@ int sb_raw_table_decode_ranges_device_ws(const void* const* d_tables, const uint
     if (rc) return rc;
     ok(err);
     return 0;
+}
+
+uint64_t sb_frame_table_gather_scratch_bytes(uint32_t nranges) {
+    return sbk::k17_carve<sbk::TablePlan>(nullptr, nranges, nullptr);
+}
+int sb_frame_table_gather_device_ws(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens,
+                                    uint32_t count, const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len,
+                                    uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
+                                    uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
+    return gather_call<sbk::TablePlan>(d_tables, d_ins, d_in_lens, count, d_unit, d_lo, d_len, d_out_ptrs, d_out_lens,
+                                       d_statuses, nranges, scratch, scratch_bytes, stream, err, launch_frame_table_gather);
+}
+uint64_t sb_raw_table_gather_scratch_bytes(uint32_t nranges) {
+    return sbk::k17_carve<sbk::RawRangePlan>(nullptr, nranges, nullptr);
+}
+int sb_raw_table_gather_device_ws(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens,
+                                  uint32_t count, const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len,
+                                  uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
+                                  uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
+    return gather_call<sbk::RawRangePlan>(d_tables, d_ins, d_in_lens, count, d_unit, d_lo, d_len, d_out_ptrs, d_out_lens,
+                                          d_statuses, nranges, scratch, scratch_bytes, stream, err, launch_raw_table_gather);
 }
 
 int sb_compress(const uint8_t* in, size_t n, uint8_t* out, size_t cap, size_t* out_n, sb_error* err) {

@@ -3,7 +3,7 @@ import ctypes as C
 
 from . import _lib
 from .error import from_c
-from .raw import _batch_encode, _ptr, _stored_tables
+from .raw import _batch_encode, _check_ranges, _gather, _gathered, _ptr, _stored_tables
 
 MAX_BLOCK_SIZE = 1 << 16                      # src/lib.rs:97
 MAX_COMPRESS_BLOCK_SIZE = 76490               # src/frame.rs:12
@@ -468,3 +468,20 @@ class TableReader:
             out += [back[o:o + int(m)].tobytes() for o, m in zip(offs, lens)]
             a = b
         return out
+
+    def gather(self, ranges):
+        """Every (i, lo, n) range of stream i gathered on the device: (data, offsets), data one CUDA uint8 tensor with
+        the ranges back to back and offsets an int64 array of len(ranges) + 1 entries, data[offsets[j]:offsets[j + 1]]
+        being read_ranges(ranges)[j]. Ranges may be as read_ranges takes them. The calls
+        (sb_frame_table_gather_device_ws) decode a chunk shared by many ranges as an edge once per call, and take up to
+        GATHER_RANGES_PER_CALL ranges and BYTES_PER_CALL output bytes each. Raises the first failing range's error, as
+        read_ranges does."""
+        import torch
+        ranges = _check_ranges(ranges, len(self._ins))
+        rooms = [max(0, min(n, self.lengths[i] - lo)) for i, lo, n in ranges]
+        offs = _gathered(rooms)
+        data = torch.empty(int(offs[-1]), dtype=torch.uint8, device=self._dev)
+        bad = _gather(self, "frame", ranges, rooms, data, offs[:-1]) if ranges else None
+        if bad:
+            raise bad[1]
+        return data, offs

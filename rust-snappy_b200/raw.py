@@ -203,6 +203,68 @@ def _stored_tables(tables, lens, dev, magic, rec, records):
     return out, words
 
 
+GATHER_RANGES_PER_CALL = 1 << 20            # ranges one gather call takes: its scratch is 108 bytes each plus 256 MiB
+
+
+def _check_ranges(ranges, count):
+    """Ranges as (stream, lo, n) ints; IndexError or ValueError as read_ranges raises them."""
+    ranges = [(int(i), int(lo), int(n)) for i, lo, n in ranges]
+    for i, lo, n in ranges:
+        if not 0 <= i < count:
+            raise IndexError("stream %d of %d" % (i, count))
+        if lo < 0 or n < 0 or lo + n > 0xFFFFFFFFFFFFFFFF:
+            raise ValueError("range (%d, %d) is not within 64-bit offsets" % (lo, n))
+    return ranges
+
+
+def _gather(reader, fmt, ranges, rooms, data, offs):
+    """sb_{fmt}_table_gather_device_ws over `ranges` (stream, lo, n) of a TableReader, each into data[offs[j]:] (rooms[j]
+    bytes), in calls of at most GATHER_RANGES_PER_CALL ranges and BYTES_PER_CALL output bytes (a single larger range gets
+    its own call). Returns the first failing range (its index in `ranges`) and its error, or None."""
+    import numpy as np
+    import torch
+    L = _lib.lib()
+    scratch_bytes = getattr(L, "sb_%s_table_gather_scratch_bytes" % fmt)
+    call = getattr(L, "sb_%s_table_gather_device_ws" % fmt)
+    a, k = 0, len(ranges)
+    rooms = np.asarray(rooms, dtype=np.int64)
+    ends = np.cumsum(rooms)
+    while a < k:
+        b = min(k, a + GATHER_RANGES_PER_CALL)
+        base = int(ends[a - 1]) if a else 0
+        b = max(a + 1, min(b, int(np.searchsorted(ends, base + reader.BYTES_PER_CALL, side="right"))))
+        part = ranges[a:b]
+        m = b - a
+        desc = np.concatenate([np.array([lo for _, lo, _ in part] + [n for _, _, n in part], dtype=np.uint64).view(np.int64),
+                               np.asarray(offs[a:b], dtype=np.int64) + data.data_ptr()])
+        t_desc = torch.from_numpy(desc).to(reader._dev)
+        t_unit = torch.from_numpy(np.array([i for i, _, _ in part] + [0], dtype=np.uint32).view(np.int32)).to(reader._dev)
+        t_res = torch.zeros(5 * m, dtype=torch.int64, device=reader._dev)       # out_lens, statuses
+        need = scratch_bytes(m)
+        scr = torch.empty(need, dtype=torch.uint8, device=reader._dev)
+        e = _lib.SbError()
+        p = t_desc.data_ptr()
+        if call(reader._t_tables.data_ptr(), reader._t_ins.data_ptr(), reader._t_lens.data_ptr(), len(reader._ins),
+                t_unit.data_ptr(), p, p + 8 * m, p + 16 * m, t_res.data_ptr(), t_res.data_ptr() + 8 * m, m,
+                scr.data_ptr(), need, reader._cuda, C.byref(e)):
+            raise from_c(e)
+        sts = t_res[m:].cpu().numpy().view(np.uint64).reshape(m, 4)
+        bad = np.nonzero(sts[:, 0] & 0xFFFFFFFF)[0]
+        if bad.size:
+            s = sts[int(bad[0])]
+            return a + int(bad[0]), from_c(_lib.SbError(int(s[0] & 0xFFFFFFFF), 0, int(s[1]), int(s[2]), int(s[3])))
+        a = b
+    return None
+
+
+def _gathered(rooms):
+    """The offsets of ranges packed back to back: len(rooms) + 1 int64 entries."""
+    import numpy as np
+    offs = np.zeros(len(rooms) + 1, dtype=np.int64)
+    offs[1:] = np.cumsum(np.asarray(rooms, dtype=np.int64))
+    return offs
+
+
 class TableReader:
     """Random access to the decoded bytes of many raw streams on the device. Each stream gets a seek table, built once on
     the device in batch calls (sb_raw_table_build_batch_device_ws), one per group of streams whatever their number: the
@@ -346,9 +408,9 @@ class TableReader:
         back = t_res.cpu().numpy().view(np.uint64)
         return back[:k], back[k:5 * k].reshape(k, 4), t_out, offs
 
-    def _decode_whole(self, which):
+    def _decode_whole(self, which, device=False):
         """Streams that are not seekable, each as Decoder().decompress_vec gives it: {stream: bytes or the exception},
-        the decodable ones in one sb_decompress_batch_device_ws call."""
+        the decodable ones in one sb_decompress_batch_device_ws call. device: the bytes as CUDA uint8 tensors."""
         import numpy as np
         import torch
         L = _lib.lib()
@@ -381,11 +443,11 @@ class TableReader:
         if L.sb_decompress_batch_device_ws(C.byref(b), in_bytes, None, scr.data_ptr(), need, self._cuda, C.byref(e)):
             raise from_c(e)
         st = t_res.cpu().numpy().view(np.uint64)[k:].reshape(k, 4)
-        back = t_out.cpu().numpy()
+        back = t_out if device else t_out.cpu().numpy()
         for j, (i, dn) in enumerate(todo):
             s = st[j]
             got[i] = from_c(_lib.SbError(int(s[0] & 0xFFFFFFFF), 0, int(s[1]), int(s[2]), int(s[3]))) \
-                if s[0] & 0xFFFFFFFF else back[at[j]:at[j] + dn].tobytes()
+                if s[0] & 0xFFFFFFFF else back[at[j]:at[j] + dn] if device else back[at[j]:at[j] + dn].tobytes()
         return got
 
     def read(self, i: int, lo: int, n: int) -> bytes:
@@ -427,3 +489,36 @@ class TableReader:
                 raise r
             out.append(r[lo:lo + n] if not self.seekable[i] else r)
         return out
+
+    def gather(self, ranges):
+        """Every (i, lo, n) range of stream i gathered on the device: (data, offsets), data one CUDA uint8 tensor with
+        the ranges back to back and offsets an int64 array of len(ranges) + 1 entries, data[offsets[j]:offsets[j + 1]]
+        being read_ranges(ranges)[j]. Ranges may be as read_ranges takes them; the ranges of seekable streams go through
+        sb_raw_table_gather_device_ws, which decodes a block shared by many ranges as an edge once per call, in calls of
+        up to GATHER_RANGES_PER_CALL ranges and BYTES_PER_CALL output bytes. A stream that is not seekable is decoded
+        whole once and sliced on the device. Raises the first failing range's error, as read_ranges does."""
+        import torch
+        ranges = _check_ranges(ranges, len(self._ins))
+        whole = self._decode_whole(sorted({i for i, _, _ in ranges if not self.seekable[i]}), device=True)
+        rooms = []
+        for i, lo, n in ranges:
+            w = whole.get(i)
+            size = w.numel() if isinstance(w, torch.Tensor) else self.lengths[i] if self.seekable[i] else 0
+            rooms.append(max(0, min(n, size - lo)))
+        offs = _gathered(rooms)
+        data = torch.empty(int(offs[-1]), dtype=torch.uint8, device=self._dev)
+        tabled = [j for j, (i, _, _) in enumerate(ranges) if self.seekable[i]]
+        bad = _gather(self, "raw", [ranges[j] for j in tabled], [rooms[j] for j in tabled], data, offs[tabled]) \
+            if tabled else None
+        first, err = (tabled[bad[0]], bad[1]) if bad else (len(ranges), None)
+        for j, (i, lo, n) in enumerate(ranges):
+            if self.seekable[i]:
+                continue
+            if isinstance(whole[i], Exception):
+                if j < first:
+                    raise whole[i]
+            elif rooms[j]:
+                data[int(offs[j]):int(offs[j + 1])].copy_(whole[i][lo:lo + rooms[j]])
+        if err is not None:
+            raise err
+        return data, offs
