@@ -492,6 +492,38 @@ int sb_raw_table_gather_device_ws(const void* const* d_tables, const uint8_t* co
                                   uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
                                   uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
 
+/* Gathers over streams that stay in host memory. The arguments are exactly those of sb_frame_table_gather_device_ws /
+ * sb_raw_table_gather_device_ws, and every range gets the status, out_len and bytes that call gives it over the same
+ * tables and the same stream bytes. Nothing is written outside [out_r, out_r + max(end - lo, 0)) or the scratch, and the
+ * call rules and SB_E_INVALID checks are the device gather's. The difference: d_ins[u] may be any address the device
+ * reads at the same value, that is page-locked host memory mapped into the device's address space (cudaHostAlloc /
+ * cudaMallocHost, torch pin_memory, cudaHostRegister) or device memory. sb_host_stream_check tells which addresses
+ * qualify. Pageable host memory is undefined behaviour (a device fault) and must not be passed.
+ * Cost: the warp that decodes a chunk or block first copies its compressed body from stream memory into a compressed
+ * slot of its own, in 16-byte loads, and decodes from there. Each body the call decodes is read from stream memory once
+ * per decode: an edge once per work item of at most 256 ranges, an interior chunk or block once per range holding it.
+ * No other stream byte is read, with two exceptions that read in place: a raw block whose compressed bytes do not fit
+ * a slot (only a wasteful encoder writes one; a legal block may spend 5 bytes per output byte), and the re-decode that
+ * finds a failing chunk's status. The tables, outputs, ranges and scratch are device memory.
+ * Scratch, exactly: sb_*_table_gather_scratch_bytes(nranges) + min(2 * nranges, 4096) * 76,544 bytes (one slot of
+ * 76,490 bytes, the largest frame chunk body, rounded up to 256, per pool warp): at most
+ * 128 * nranges + 4096 * (65,536 + 76,544) + 64 KiB bytes whatever the streams hold. */
+uint64_t sb_frame_table_gather_host_streams_scratch_bytes(uint32_t nranges);
+int sb_frame_table_gather_host_streams_ws(const void* const* d_tables, const uint8_t* const* d_ins,
+                                          const uint64_t* d_in_lens, uint32_t count, const uint32_t* d_unit,
+                                          const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                                          uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
+                                          uint64_t scratch_bytes, void* stream, sb_error* err);
+uint64_t sb_raw_table_gather_host_streams_scratch_bytes(uint32_t nranges);
+int sb_raw_table_gather_host_streams_ws(const void* const* d_tables, const uint8_t* const* d_ins,
+                                        const uint64_t* d_in_lens, uint32_t count, const uint32_t* d_unit,
+                                        const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                                        uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
+                                        uint64_t scratch_bytes, void* stream, sb_error* err);
+/* Host only, no launch: Ok when p and p + n - 1 are both readable by the current device at the same address (page-locked
+ * host memory mapped at that address, or device memory); n == 0 is Ok. Otherwise SB_E_INVALID{a = p, b = n, c = 6}. */
+int sb_host_stream_check(const void* p, uint64_t n, sb_error* err);
+
 /* Batch encoders that also write one seek table per unit, so what they write is seekable without a build. Each does
  * exactly what its untabled call does: output bytes, out_lens, statuses and (frame) d_chunk_offs are byte-identical to
  * sb_compress_batch_device_ws / sb_frame_encode_batch_device_ws with the same arguments, rejected units and the in_bytes

@@ -48,6 +48,8 @@ SYMBOLS = [
     "sb_raw_table_build_batch_device_ws", "sb_raw_table_ranges_scratch_bytes", "sb_raw_table_decode_ranges_device_ws",
     "sb_frame_table_gather_scratch_bytes", "sb_frame_table_gather_device_ws", "sb_raw_table_gather_scratch_bytes",
     "sb_raw_table_gather_device_ws",
+    "sb_frame_table_gather_host_streams_scratch_bytes", "sb_frame_table_gather_host_streams_ws",
+    "sb_raw_table_gather_host_streams_scratch_bytes", "sb_raw_table_gather_host_streams_ws", "sb_host_stream_check",
     "sb_compress_tables_bytes", "sb_compress_batch_tabled_scratch_bytes", "sb_compress_batch_tabled_device_ws",
     "sb_frame_encode_tables_bytes", "sb_frame_encode_batch_tabled_scratch_bytes", "sb_frame_encode_batch_tabled_device_ws",
     "sb_frame_max_len", "sb_frame_encode", "sb_frame_encode_ex", "sb_frame_decode", "sb_frame_encode_device",
@@ -140,6 +142,11 @@ def lib():
         getattr(L, "sb_%s_table_gather_scratch_bytes" % fmt).argtypes = [C.c_uint32]
         getattr(L, "sb_%s_table_gather_device_ws" % fmt).argtypes = [vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp, vp,
                                                                      C.c_uint32, vp, C.c_uint64, vp, ep]
+        getattr(L, "sb_%s_table_gather_host_streams_scratch_bytes" % fmt).restype = C.c_uint64
+        getattr(L, "sb_%s_table_gather_host_streams_scratch_bytes" % fmt).argtypes = [C.c_uint32]
+        getattr(L, "sb_%s_table_gather_host_streams_ws" % fmt).argtypes = [vp, vp, vp, C.c_uint32, vp, vp, vp, vp, vp,
+                                                                           vp, C.c_uint32, vp, C.c_uint64, vp, ep]
+    L.sb_host_stream_check.argtypes = [vp, C.c_uint64, ep]
     for name in ("sb_compress_tables_bytes", "sb_compress_batch_tabled_scratch_bytes", "sb_frame_encode_tables_bytes",
                  "sb_frame_encode_batch_tabled_scratch_bytes"):
         getattr(L, name).restype = C.c_uint64

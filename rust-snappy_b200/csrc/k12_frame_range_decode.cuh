@@ -31,6 +31,7 @@
 #pragma once
 #include "k5_frame_decode.cuh"
 #include "k8_raw_split.cuh"
+#include "k18_host_gather.cuh"
 
 namespace sbk {
 

@@ -151,16 +151,21 @@ SB_DEVICE void k13_plan_tiles_body(const TablePlan& q) { scan_tiles_body(q.nrang
 // GATHER (the gather call, k17_table_gather.cuh): only pairs inside [lo, end) decode here, on the whole grid. The head
 // and tail pairs that are not inside are left to K17's gather decode. A middle pair that is not inside (only a table
 // whose offsets were tampered with has one) sets rec[r]._pad, and the gather's finish walks that range's run for it.
-template <bool GATHER = false>
-SB_DEVICE void k13_decode_body(const TablePlan& q) {
+// HOST (the host-stream gather, k18_host_gather.cuh): only the pool's warps decode, warp w fetching each body into its
+// compressed slot cpool + w * K18_CSLOT first.
+template <bool GATHER = false, bool HOST = false>
+SB_DEVICE void k13_decode_body(const TablePlan& q, uint8_t* cpool = nullptr) {
     uint32_t* tab = (uint32_t*)smem();                                // K3 slicing tables (4 KB)
     k3_build_tables(tab);
     uint32_t* elems = (uint32_t*)(smem() + K3_TABLE_BYTES) + warp_id() * 64;
     const unsigned wpb = block_dim() >> 5;
     sb_error* sink = (sb_error*)(smem() + K3_TABLE_BYTES + wpb * K2_SMEM_PER_WARP) + warp_id();
     const uint64_t pairs = k8b_at(q.pr_offs, q.pr_tiles, q.nranges);
-    const uint64_t nwarps = (uint64_t)grid_dim() * wpb;
-    for (uint64_t g = (uint64_t)block_idx() * wpb + warp_id(); g < pairs; g += nwarps) {
+    uint64_t nwarps = (uint64_t)grid_dim() * wpb;
+    const uint64_t w = (uint64_t)block_idx() * wpb + warp_id();
+    if (HOST) { nwarps = k12_pool_warps(nwarps, q.nranges); if (w >= nwarps) return; }
+    uint8_t* const cslot = HOST ? cpool + w * K18_CSLOT : nullptr;
+    for (uint64_t g = w; g < pairs; g += nwarps) {
         const uint32_t r = k8b_unit_of(q.pr_offs, q.pr_tiles, q.nranges, g);
         const uint32_t first = q.rec[r].first, k = first + (uint32_t)(g - k8b_at(q.pr_offs, q.pr_tiles, r));
         const uint32_t u = q.unit[r];                                    // a range with pairs passed k13_head
@@ -177,7 +182,10 @@ SB_DEVICE void k13_decode_body(const TablePlan& q) {
             }
             uint8_t* dst = inside ? q.outs[r] + (t.off - lo) : q.staging + ((uint64_t)r * 2 + (k == first ? 0 : 1)) * K12_SLOT;
             if (GATHER) K17_COUNT_DECODE();
-            code = k5_decode_chunk(tab, elems, k13_chunk(t), q.ins[u], dst, sink);
+            FChunk c = k13_chunk(t);
+            const uint8_t* in = q.ins[u];
+            if (HOST) { in = k18_body<true>(in + t.body_off, t.body_len, cslot); c.body_off = 0; }
+            code = k5_decode_chunk(tab, elems, c, in, dst, sink);
             if (code == SB_OK && !inside) {                               // the slice of [lo, end) a head or tail chunk holds
                 const uint64_t a = t.off > lo ? t.off : lo, e = t.off + t.dlen < end ? t.off + t.dlen : end;
                 warp_copy(q.outs[r] + (a - lo), dst + (a - t.off), (uint32_t)(e - a));

@@ -295,16 +295,20 @@ SB_DEVICE void k15_plan_tiles_body(const RawRangePlan& q) { scan_tiles_body(q.nr
 
 // GATHER (the gather call, k17_table_gather.cuh): the head and tail pairs that are not inside [lo, end) are left to K17's
 // gather decode (only they can straddle lo or end: blocks are implied by their index), so no warp needs staging and
-// the whole grid decodes.
-template <bool GATHER = false>
-SB_DEVICE void k15_decode_body(const RawRangePlan& q) {
+// the whole grid decodes. HOST (the host-stream gather, k18_host_gather.cuh): only the pool's warps decode, warp w
+// fetching each body that fits into its compressed slot cpool + w * K18_CSLOT first.
+template <bool GATHER = false, bool HOST = false>
+SB_DEVICE void k15_decode_body(const RawRangePlan& q, uint8_t* cpool = nullptr) {
     uint32_t* tab = (uint32_t*)smem();                                // K3 slicing tables (4 KB)
     k3_build_tables(tab);
     uint32_t* elems = (uint32_t*)(smem() + K3_TABLE_BYTES) + warp_id() * 64;
     const unsigned wpb = block_dim() >> 5;
     const uint64_t pairs = k8b_at(q.pr_offs, q.pr_tiles, q.nranges);
-    const uint64_t nwarps = (uint64_t)grid_dim() * wpb;
-    for (uint64_t g = (uint64_t)block_idx() * wpb + warp_id(); g < pairs; g += nwarps) {
+    uint64_t nwarps = (uint64_t)grid_dim() * wpb;
+    const uint64_t w = (uint64_t)block_idx() * wpb + warp_id();
+    if (HOST) { nwarps = k12_pool_warps(nwarps, q.nranges); if (w >= nwarps) return; }
+    uint8_t* const cslot = HOST ? cpool + w * K18_CSLOT : nullptr;
+    for (uint64_t g = w; g < pairs; g += nwarps) {
         const uint32_t r = k8b_unit_of(q.pr_offs, q.pr_tiles, q.nranges, g);
         const uint32_t first = q.rec[r].first, j = first + (uint32_t)(g - k8b_at(q.pr_offs, q.pr_tiles, r));
         const uint32_t u = q.unit[r];                                    // a range with pairs passed k15_head
@@ -319,7 +323,8 @@ SB_DEVICE void k15_decode_body(const RawRangePlan& q) {
             if (GATHER && !inside) { syncwarp(); continue; }
             uint8_t* dst = inside ? q.outs[r] + (off - lo) : q.staging + ((uint64_t)r * 2 + (j == first ? 0 : 1)) * K12_SLOT;
             if (GATHER) K17_COUNT_DECODE();
-            code = k2_decode_stream<false>(q.ins[u] + a, b - a, dst, dl, nullptr, nullptr, elems);
+            if (HOST) code = k2_decode_stream<false>(k18_body<true>(q.ins[u] + a, b - a, cslot), b - a, dst, dl, nullptr, nullptr, elems);
+            else code = k2_decode_stream<false>(q.ins[u] + a, b - a, dst, dl, nullptr, nullptr, elems);
             syncwarp();
             if (code == SB_OK && k3_warp_crc32c_masked(tab, dst, (uint32_t)dl) != t[j].crc) code = SB_CHECKSUM;
             if (code == SB_OK && !inside) {                               // the slice of [lo, end) a head or tail block holds

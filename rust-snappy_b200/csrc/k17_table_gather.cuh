@@ -186,8 +186,10 @@ SB_DEVICE GatherItem k17_item(const GatherPlan<P>& g, uint64_t i) {
     return it;
 }
 
-// ---- gather decode: warp w of the pool's warps on slot w
-SB_DEVICE void k17_frame_gather_body(const GatherPlan<TablePlan>& g) {
+// ---- gather decode: warp w of the pool's warps on slot w. HOST (k18_host_gather.cuh): the edge's body is fetched into
+// the warp's compressed slot cpool + w * K18_CSLOT first.
+template <bool HOST = false>
+SB_DEVICE void k17_frame_gather_body(const GatherPlan<TablePlan>& g, uint8_t* cpool = nullptr) {
     const TablePlan& q = g.q;
     uint32_t* tab = (uint32_t*)smem();                                // K3 slicing tables (4 KB)
     k3_build_tables(tab);
@@ -198,6 +200,7 @@ SB_DEVICE void k17_frame_gather_body(const GatherPlan<TablePlan>& g) {
     const uint64_t nw = k12_pool_warps((uint64_t)grid_dim() * wpb, q.nranges);
     if (w >= nw) return;
     uint8_t* slot = q.staging + w * K12_SLOT;
+    uint8_t* const cslot = HOST ? cpool + w * K18_CSLOT : nullptr;
     const uint64_t items = k8b_at(g.i_offs, g.i_tiles, g.nh);
     for (uint64_t i = w; i < items; i += nw) {
         const GatherItem it = k17_item(g, i);
@@ -206,7 +209,10 @@ SB_DEVICE void k17_frame_gather_body(const GatherPlan<TablePlan>& g) {
         const TableHead* h = (const TableHead*)q.tables[u];
         const TableRec t = k13_recs(h)[k];                              // its bounds passed k13_rec_ok at the insert
         K17_COUNT_DECODE();
-        const uint32_t code = k5_decode_chunk(tab, elems, k13_chunk(t), q.ins[u], slot, sink);
+        FChunk c = k13_chunk(t);
+        const uint8_t* in = q.ins[u];
+        if (HOST) { in = k18_body<true>(in + t.body_off, t.body_len, cslot); c.body_off = 0; }
+        const uint32_t code = k5_decode_chunk(tab, elems, c, in, slot, sink);
         for (uint64_t e = it.a; e < it.b; e++) {
             const uint32_t r = g.list[e] >> 1;
             if (code != SB_OK) { if (lane_id() == 0) atomic_min(&q.rec[r].first_bad, k); continue; }
@@ -218,7 +224,8 @@ SB_DEVICE void k17_frame_gather_body(const GatherPlan<TablePlan>& g) {
     }
 }
 
-SB_DEVICE void k17_raw_gather_body(const GatherPlan<RawRangePlan>& g) {
+template <bool HOST = false>
+SB_DEVICE void k17_raw_gather_body(const GatherPlan<RawRangePlan>& g, uint8_t* cpool = nullptr) {
     const RawRangePlan& q = g.q;
     uint32_t* tab = (uint32_t*)smem();                                // K3 slicing tables (4 KB)
     k3_build_tables(tab);
@@ -228,6 +235,7 @@ SB_DEVICE void k17_raw_gather_body(const GatherPlan<RawRangePlan>& g) {
     const uint64_t nw = k12_pool_warps((uint64_t)grid_dim() * wpb, q.nranges);
     if (w >= nw) return;
     uint8_t* slot = q.staging + w * K12_SLOT;
+    uint8_t* const cslot = HOST ? cpool + w * K18_CSLOT : nullptr;
     const uint64_t items = k8b_at(g.i_offs, g.i_tiles, g.nh);
     for (uint64_t i = w; i < items; i += nw) {
         const GatherItem it = k17_item(g, i);
@@ -238,7 +246,9 @@ SB_DEVICE void k17_raw_gather_body(const GatherPlan<RawRangePlan>& g) {
         const uint64_t off = (uint64_t)j << 16, dl = h->dn - off < 65536 ? h->dn - off : 65536;
         const uint32_t a = t[j].off, b = j + 1 < h->nblocks ? t[j + 1].off : (uint32_t)h->n;
         K17_COUNT_DECODE();
-        uint32_t code = k2_decode_stream<false>(q.ins[u] + a, b - a, slot, dl, nullptr, nullptr, elems);
+        const uint8_t* in = q.ins[u] + a;
+        if (HOST) in = k18_body<true>(in, b - a, cslot);
+        uint32_t code = k2_decode_stream<false>(in, b - a, slot, dl, nullptr, nullptr, elems);
         syncwarp();
         if (code == SB_OK && k3_warp_crc32c_masked(tab, slot, (uint32_t)dl) != t[j].crc) code = SB_CHECKSUM;
         for (uint64_t e = it.a; e < it.b; e++) {

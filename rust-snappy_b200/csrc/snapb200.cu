@@ -158,6 +158,20 @@ __global__ void __launch_bounds__(128, 4) k17_raw_interior_kernel(sbk::RawRangeP
 __global__ void __launch_bounds__(128, 8) k17_frame_gather_kernel(sbk::GatherPlan<sbk::TablePlan> g) { sbk::k17_frame_gather_body(g); }
 __global__ void __launch_bounds__(128, 8) k17_raw_gather_kernel(sbk::GatherPlan<sbk::RawRangePlan> g) { sbk::k17_raw_gather_body(g); }
 __global__ void __launch_bounds__(128) k17_frame_finish_kernel(sbk::TablePlan q) { sbk::k13_finish_body<true>(q); }
+// the host-stream gathers (K18): interior and edge decodes on the pool's warps, each fetching a body into its
+// compressed slot before it decodes; 8 CTAs of 128 per SM, so that the pool's 4,096 warps all run
+__global__ void __launch_bounds__(128, 8) k18_frame_interior_kernel(sbk::TablePlan q, uint8_t* cpool) {
+    sbk::k13_decode_body<true, true>(q, cpool);
+}
+__global__ void __launch_bounds__(128, 8) k18_raw_interior_kernel(sbk::RawRangePlan q, uint8_t* cpool) {
+    sbk::k15_decode_body<true, true>(q, cpool);
+}
+__global__ void __launch_bounds__(128, 8) k18_frame_gather_kernel(sbk::GatherPlan<sbk::TablePlan> g, uint8_t* cpool) {
+    sbk::k17_frame_gather_body<true>(g, cpool);
+}
+__global__ void __launch_bounds__(128, 8) k18_raw_gather_kernel(sbk::GatherPlan<sbk::RawRangePlan> g, uint8_t* cpool) {
+    sbk::k17_raw_gather_body<true>(g, cpool);
+}
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
@@ -933,7 +947,8 @@ int launch_raw_table_ranges(Ctx& c, const sbk::RawRangePlan& q, cudaStream_t st,
 
 
 // ---- gathers over tabled frame and raw streams (K17): the range plan, the edge lists, the interior decode, the gather
-// decode over the pool, the finish. 10 launches.
+// decode over the pool, the finish. 10 launches. cpool (the host-stream gathers, K18): the pool's compressed slots, and
+// the interior and gather decodes are K18's, on the pool's warps.
 template <class P>
 int launch_gather_lists(Ctx& c, const sbk::GatherPlan<P>& g, cudaStream_t st, sb_error* err) {
     const unsigned stiles = (unsigned)(((uint64_t)g.nh + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
@@ -946,7 +961,8 @@ int launch_gather_lists(Ctx& c, const sbk::GatherPlan<P>& g, cudaStream_t st, sb
     CK(cudaGetLastError());
     return 0;
 }
-int launch_frame_table_gather(Ctx& c, const sbk::GatherPlan<sbk::TablePlan>& g, cudaStream_t st, sb_error* err) {
+int launch_frame_table_gather(Ctx& c, const sbk::GatherPlan<sbk::TablePlan>& g, uint8_t* cpool, cudaStream_t st,
+                              sb_error* err) {
     const sbk::TablePlan& q = g.q;
     const uint64_t most = (uint64_t)16 * c.sms, fw = ((uint64_t)q.nranges + 3) / 4, slots = sbk::k17_pool_slots(q.nranges);
     const unsigned ptiles = (unsigned)(((uint64_t)q.nranges + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
@@ -956,14 +972,21 @@ int launch_frame_table_gather(Ctx& c, const sbk::GatherPlan<sbk::TablePlan>& g, 
     g_launches += 2;
     int rc = launch_gather_lists(c, g, st, err);
     if (rc) return rc;
-    k17_frame_interior_kernel<<<(unsigned)most, 128, smem + 4 * sizeof(sb_error), st>>>(q);
-    k17_frame_gather_kernel<<<(unsigned)((slots + 3) / 4), 128, smem + 4 * sizeof(sb_error), st>>>(g);
+    const unsigned pool = (unsigned)((slots + 3) / 4);
+    if (cpool) {
+        k18_frame_interior_kernel<<<pool, 128, smem + 4 * sizeof(sb_error), st>>>(q, cpool);
+        k18_frame_gather_kernel<<<pool, 128, smem + 4 * sizeof(sb_error), st>>>(g, cpool);
+    } else {
+        k17_frame_interior_kernel<<<(unsigned)most, 128, smem + 4 * sizeof(sb_error), st>>>(q);
+        k17_frame_gather_kernel<<<pool, 128, smem + 4 * sizeof(sb_error), st>>>(g);
+    }
     k17_frame_finish_kernel<<<fw < most ? (unsigned)fw : (unsigned)most, 128, smem, st>>>(q);
     g_launches += 3;
     CK(cudaGetLastError());
     return 0;
 }
-int launch_raw_table_gather(Ctx& c, const sbk::GatherPlan<sbk::RawRangePlan>& g, cudaStream_t st, sb_error* err) {
+int launch_raw_table_gather(Ctx& c, const sbk::GatherPlan<sbk::RawRangePlan>& g, uint8_t* cpool, cudaStream_t st,
+                            sb_error* err) {
     const sbk::RawRangePlan& q = g.q;
     const unsigned ptiles = (unsigned)(((uint64_t)q.nranges + 1 + sbk::K4_TILE - 1) / sbk::K4_TILE);
     const uint64_t slots = sbk::k17_pool_slots(q.nranges);
@@ -973,12 +996,25 @@ int launch_raw_table_gather(Ctx& c, const sbk::GatherPlan<sbk::RawRangePlan>& g,
     g_launches += 2;
     int rc = launch_gather_lists(c, g, st, err);
     if (rc) return rc;
-    k17_raw_interior_kernel<<<16 * c.sms, 128, smem, st>>>(q);
-    k17_raw_gather_kernel<<<(unsigned)((slots + 3) / 4), 128, smem, st>>>(g);
+    const unsigned pool = (unsigned)((slots + 3) / 4);
+    if (cpool) {
+        k18_raw_interior_kernel<<<pool, 128, smem, st>>>(q, cpool);
+        k18_raw_gather_kernel<<<pool, 128, smem, st>>>(g, cpool);
+    } else {
+        k17_raw_interior_kernel<<<16 * c.sms, 128, smem, st>>>(q);
+        k17_raw_gather_kernel<<<pool, 128, smem, st>>>(g);
+    }
     k15_finish_kernel<<<device_grid(c, q.nranges, 256, 16), 256, 0, st>>>(q);
     g_launches += 3;
     CK(cudaGetLastError());
     return 0;
+}
+
+// the scratch of a gather: the device gather's, and with host streams one compressed slot per pool warp after it
+template <class P>
+uint64_t gather_scratch(uint32_t nranges, bool host) {
+    const uint64_t bytes = sbk::k17_carve<P>(nullptr, nranges, nullptr);
+    return host ? sbk::k18_carve(nullptr, bytes, sbk::k17_pool_slots(nranges), nullptr) : bytes;
 }
 
 // the call checks of the range calls, with the gathers' range limit and scratch
@@ -986,14 +1022,14 @@ template <class P>
 int gather_call(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens, uint32_t count,
                 const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
                 uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch, uint64_t scratch_bytes,
-                void* stream, sb_error* err,
-                int (*launch)(Ctx&, const sbk::GatherPlan<P>&, cudaStream_t, sb_error*)) {
+                void* stream, sb_error* err, bool host,
+                int (*launch)(Ctx&, const sbk::GatherPlan<P>&, uint8_t*, cudaStream_t, sb_error*)) {
     if (count >= sbk::K13_MAX_COUNT) return fail(err, SB_E_INVALID, count, sbk::K13_MAX_COUNT);
     if (nranges > sbk::K17_MAX_RANGES) return fail(err, SB_E_INVALID, nranges, sbk::K17_MAX_RANGES);
     if (nranges == 0) { ok(err); return 0; }
     if (count && (!d_tables || !d_ins || !d_in_lens)) return fail(err, SB_E_INVALID);
     if (!d_unit || !d_lo || !d_len || !d_out_ptrs || !d_out_lens || !d_statuses || !scratch) return fail(err, SB_E_INVALID);
-    const uint64_t need = sbk::k17_carve<P>(nullptr, nranges, nullptr);
+    const uint64_t need = gather_scratch<P>(nranges, host);
     if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
     Ctx* c;
     int rc = get_ctx(&c, err);
@@ -1003,8 +1039,10 @@ int gather_call(const void* const* d_tables, const uint8_t* const* d_ins, const 
     P& q = g.q;
     q.tables = d_tables; q.ins = d_ins; q.in_lens = d_in_lens; q.count = count;
     q.unit = d_unit; q.lo = d_lo; q.len = d_len; q.outs = d_out_ptrs; q.out_lens = d_out_lens; q.statuses = d_statuses;
-    sbk::k17_carve(scratch, nranges, &g);
-    rc = launch(*c, g, (cudaStream_t)stream, err);
+    const uint64_t bytes = sbk::k17_carve(scratch, nranges, &g);
+    uint8_t* cpool = nullptr;
+    if (host) sbk::k18_carve(scratch, bytes, sbk::k17_pool_slots(nranges), &cpool);
+    rc = launch(*c, g, cpool, (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;
@@ -1389,25 +1427,58 @@ int sb_raw_table_decode_ranges_device_ws(const void* const* d_tables, const uint
     return 0;
 }
 
-uint64_t sb_frame_table_gather_scratch_bytes(uint32_t nranges) {
-    return sbk::k17_carve<sbk::TablePlan>(nullptr, nranges, nullptr);
-}
+uint64_t sb_frame_table_gather_scratch_bytes(uint32_t nranges) { return gather_scratch<sbk::TablePlan>(nranges, false); }
 int sb_frame_table_gather_device_ws(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens,
                                     uint32_t count, const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len,
                                     uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
                                     uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
     return gather_call<sbk::TablePlan>(d_tables, d_ins, d_in_lens, count, d_unit, d_lo, d_len, d_out_ptrs, d_out_lens,
-                                       d_statuses, nranges, scratch, scratch_bytes, stream, err, launch_frame_table_gather);
+                                       d_statuses, nranges, scratch, scratch_bytes, stream, err, false, launch_frame_table_gather);
 }
-uint64_t sb_raw_table_gather_scratch_bytes(uint32_t nranges) {
-    return sbk::k17_carve<sbk::RawRangePlan>(nullptr, nranges, nullptr);
-}
+uint64_t sb_raw_table_gather_scratch_bytes(uint32_t nranges) { return gather_scratch<sbk::RawRangePlan>(nranges, false); }
 int sb_raw_table_gather_device_ws(const void* const* d_tables, const uint8_t* const* d_ins, const uint64_t* d_in_lens,
                                   uint32_t count, const uint32_t* d_unit, const uint64_t* d_lo, const uint64_t* d_len,
                                   uint8_t* const* d_out_ptrs, uint64_t* d_out_lens, sb_error* d_statuses,
                                   uint32_t nranges, void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err) {
     return gather_call<sbk::RawRangePlan>(d_tables, d_ins, d_in_lens, count, d_unit, d_lo, d_len, d_out_ptrs, d_out_lens,
-                                          d_statuses, nranges, scratch, scratch_bytes, stream, err, launch_raw_table_gather);
+                                          d_statuses, nranges, scratch, scratch_bytes, stream, err, false, launch_raw_table_gather);
+}
+
+uint64_t sb_frame_table_gather_host_streams_scratch_bytes(uint32_t nranges) {
+    return gather_scratch<sbk::TablePlan>(nranges, true);
+}
+int sb_frame_table_gather_host_streams_ws(const void* const* d_tables, const uint8_t* const* d_ins,
+                                          const uint64_t* d_in_lens, uint32_t count, const uint32_t* d_unit,
+                                          const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                                          uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
+                                          uint64_t scratch_bytes, void* stream, sb_error* err) {
+    return gather_call<sbk::TablePlan>(d_tables, d_ins, d_in_lens, count, d_unit, d_lo, d_len, d_out_ptrs, d_out_lens,
+                                       d_statuses, nranges, scratch, scratch_bytes, stream, err, true, launch_frame_table_gather);
+}
+uint64_t sb_raw_table_gather_host_streams_scratch_bytes(uint32_t nranges) {
+    return gather_scratch<sbk::RawRangePlan>(nranges, true);
+}
+int sb_raw_table_gather_host_streams_ws(const void* const* d_tables, const uint8_t* const* d_ins,
+                                        const uint64_t* d_in_lens, uint32_t count, const uint32_t* d_unit,
+                                        const uint64_t* d_lo, const uint64_t* d_len, uint8_t* const* d_out_ptrs,
+                                        uint64_t* d_out_lens, sb_error* d_statuses, uint32_t nranges, void* scratch,
+                                        uint64_t scratch_bytes, void* stream, sb_error* err) {
+    return gather_call<sbk::RawRangePlan>(d_tables, d_ins, d_in_lens, count, d_unit, d_lo, d_len, d_out_ptrs, d_out_lens,
+                                          d_statuses, nranges, scratch, scratch_bytes, stream, err, true, launch_raw_table_gather);
+}
+// one address the device reads at the same value: device memory, or page-locked host memory mapped at that address
+static bool device_readable(const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return (a.type == cudaMemoryTypeHost && a.devicePointer == p) || a.type == cudaMemoryTypeDevice;
+}
+int sb_host_stream_check(const void* p, uint64_t n, sb_error* err) {
+    if (n == 0) { ok(err); return 0; }
+    const uintptr_t a = (uintptr_t)p;
+    if (!p || a + (n - 1) < a || !device_readable(p) || !device_readable((const void*)(a + (n - 1))))
+        return fail(err, SB_E_INVALID, (uint64_t)a, n, 6);
+    ok(err);
+    return 0;
 }
 
 int sb_compress(const uint8_t* in, size_t n, uint8_t* out, size_t cap, size_t* out_n, sb_error* err) {

@@ -3,7 +3,8 @@ import ctypes as C
 
 from . import _lib
 from .error import from_c
-from .raw import _batch_encode, _check_ranges, _gather, _gathered, _ptr, _stored_tables
+from .raw import (HOST_BUILD_BYTES, _batch_encode, _check_ranges, _gather, _gathered, _host_streams, _ptr, _split,
+                  _stored_tables, _windows)
 
 MAX_BLOCK_SIZE = 1 << 16                      # src/lib.rs:97
 MAX_COMPRESS_BLOCK_SIZE = 76490               # src/frame.rs:12
@@ -262,18 +263,24 @@ class TableReader:
     tables: the streams' stored seek tables (from encode_batch(..., tables=True) or an earlier build), bytes-like or
     CUDA uint8 tensors, instead of a build. They are uploaded in one copy and no build runs; a table whose header does
     not match its stream's length raises ValueError. A table of another stream of the same length gives the reads over
-    it a chunk's checksum error, never wrong bytes."""
+    it a chunk's checksum error, never wrong bytes.
+    host: the streams stay in pinned host memory (bytes-like ones copied once into one pinned buffer, pinned CPU uint8
+    tensors kept alive; unpinned CPU and CUDA tensors raise ValueError), so a corpus larger than the device can be read.
+    Only the tables live on the device: they are built from uploads of at most HOST_BUILD_BYTES of streams at a time.
+    Reads go through sb_frame_table_gather_host_streams_ws, which copies over PCIe only the compressed chunks it
+    decodes; read_ranges is then the gather, split. Results and errors are those of a reader without host."""
 
     RANGES_PER_CALL = RangeReader.RANGES_PER_CALL
     BYTES_PER_CALL = RangeReader.BYTES_PER_CALL
 
-    def __init__(self, streams, fragment=False, tables=None):
+    def __init__(self, streams, fragment=False, tables=None, host=False):
         import numpy as np
         import torch
         self._dev = torch.device("cuda", torch.cuda.current_device())
         self._cuda = torch.cuda.current_stream(self._dev).cuda_stream
-        self._ins, host = [], []
-        for s in streams:
+        self._host = bool(host)
+        self._ins, host = ([], []) if not self._host else (_host_streams(streams), [])
+        for s in streams if not self._host else ():
             if isinstance(s, torch.Tensor):
                 if not s.is_cuda or s.dtype != torch.uint8 or s.dim() != 1 or not s.is_contiguous():
                     raise ValueError("TableReader takes contiguous 1-D CUDA uint8 tensors")
@@ -300,17 +307,22 @@ class TableReader:
             self._keep_tables([t.data_ptr() for t in self._bufs], lens)
             return
         ptrs, results = [0] * count, [None] * count
-        # a stream that fits an sb_batch unit is tabled in a batch call; a longer one gets a build of its own
-        for i, t, r in zip(*self._build([i for i in range(count) if lens[i] > 0xFFFFFFFF], flags)):
-            self._bufs.append(t)
-            ptrs[i], results[i] = t.data_ptr(), r
-        # the chunk table as RangeReader sizes it: encoder chunks hold 64 KiB, and any data chunk is at least 8 bytes.
-        # Streams that did not fit the first time are built again with the larger bound.
-        todo = [i for i in range(count) if lens[i] <= 0xFFFFFFFF]
-        for per in (1024, 8):
-            for i, p, r in self._build_batch(todo, [min(lens[i] // per + 16, MAX_BATCH_CHUNKS) for i in todo], flags):
-                ptrs[i], results[i] = p, r
-            todo = [i for i in todo if results[i].status.code == 202 and results[i].status.b == 1]
+        groups = _windows(range(count), lens, HOST_BUILD_BYTES) if self._host else [list(range(count))]
+        for g in groups:                                                 # host streams: one uploaded window at a time
+            ins = {i: self._ins[i].to(self._dev) for i in g} if self._host else self._ins
+            # a stream that fits an sb_batch unit is tabled in a batch call; a longer one gets a build of its own
+            for i, t, r in zip(*self._build([i for i in g if lens[i] > 0xFFFFFFFF], flags, ins)):
+                self._bufs.append(t)
+                ptrs[i], results[i] = t.data_ptr(), r
+            # the chunk table as RangeReader sizes it: encoder chunks hold 64 KiB, and any data chunk is at least 8
+            # bytes. Streams that did not fit the first time are built again with the larger bound.
+            todo = [i for i in g if lens[i] <= 0xFFFFFFFF]
+            for per in (1024, 8):
+                for i, p, r in self._build_batch(todo, [min(lens[i] // per + 16, MAX_BATCH_CHUNKS) for i in todo], flags,
+                                                 ins):
+                    ptrs[i], results[i] = p, r
+                todo = [i for i in todo if results[i].status.code == 202 and results[i].status.b == 1]
+            del ins
         self.lengths = [int(r.bytes) for r in results]
         self._keep_tables(ptrs, lens)
 
@@ -323,10 +335,11 @@ class TableReader:
         self._t_ins = to64([t.data_ptr() for t in self._ins] + [0])
         self._t_lens = to64(lens + [0])
 
-    def _build_batch(self, which, caps, flags):
-        """sb_frame_table_build_batch_device_ws over groups of streams whose chunk tables (caps) sum to at most
-        MAX_BATCH_CHUNKS: one call and one wait per group, whatever the number of streams. A group's tables stay in one
-        buffer cut to their packed size. Yields (stream, its table's address, its result) for every stream."""
+    def _build_batch(self, which, caps, flags, streams):
+        """sb_frame_table_build_batch_device_ws over groups of `streams` (device tensors by stream index) whose chunk
+        tables (caps) sum to at most MAX_BATCH_CHUNKS: one call and one wait per group, whatever the number of streams.
+        A group's tables stay in one buffer cut to their packed size. Yields (stream, its table's address, its result)
+        for every stream."""
         import numpy as np
         import torch
         L = _lib.lib()
@@ -342,7 +355,7 @@ class TableReader:
         rsz = C.sizeof(_lib.SbFrameResult)
         for g, max_chunks in groups:
             k = len(g)
-            ins = [self._ins[i] for i in g]
+            ins = [streams[i] for i in g]
             in_bytes = sum(t.numel() for t in ins)
             desc = np.concatenate([np.array([t.data_ptr() for t in ins], dtype=np.uint64).view(np.int64),
                                    np.array([t.numel() for t in ins] + [0] * (k % 2), dtype=np.uint32).view(np.int64)])
@@ -368,21 +381,22 @@ class TableReader:
             for j, i in enumerate(g):
                 yield i, kept.data_ptr() + int(offs[j]), _lib.SbFrameResult.from_buffer_copy(raw[j * rsz:(j + 1) * rsz])
 
-    def _build(self, which, flags):
+    def _build(self, which, flags, streams):
         """A table per stream by sb_frame_table_build_device_ws (streams too long for a batch unit), its chunk table
         sized as RangeReader sizes it and built once more when too small: (streams, tables cut to size, results)."""
         L = _lib.lib()
         if not which:
             return [], [], []
-        caps = [min(self._ins[i].numel() // 1024 + 16, MAX_BATCH_CHUNKS) for i in which]
-        tables, results = self._build_each(which, caps, flags)
+        caps = [min(streams[i].numel() // 1024 + 16, MAX_BATCH_CHUNKS) for i in which]
+        tables, results = self._build_each(which, caps, flags, streams)
         for j, i in enumerate(which):
             if results[j].status.code == 202 and results[j].status.b == 1:
-                more, res2 = self._build_each([i], [min(self._ins[i].numel() // 8 + 16, MAX_BATCH_CHUNKS)], flags)
+                more, res2 = self._build_each([i], [min(streams[i].numel() // 8 + 16, MAX_BATCH_CHUNKS)], flags,
+                                              streams)
                 tables[j], results[j] = more[0], res2[0]
         return which, [t[:L.sb_frame_table_bytes(r.nchunks)].clone() for t, r in zip(tables, results)], results
 
-    def _build_each(self, which, caps, flags):
+    def _build_each(self, which, caps, flags, streams):
         """One sb_frame_table_build_device_ws per stream, one wait for all: (tables, results)."""
         import numpy as np
         import torch
@@ -394,7 +408,7 @@ class TableReader:
         t_res = torch.zeros(max(len(which), 1) * rsz, dtype=torch.uint8, device=self._dev)
         tables = []
         for j, (i, cap) in enumerate(zip(which, caps)):
-            t_in = self._ins[i]
+            t_in = streams[i]
             tb = L.sb_frame_table_bytes(cap)
             table = torch.empty(tb, dtype=torch.uint8, device=self._dev)
             e = _lib.SbError()
@@ -443,7 +457,9 @@ class TableReader:
     def read_ranges(self, ranges) -> list:
         """One bytes object per (i, lo, n) range of stream i. Ranges may mix streams in any order and be empty,
         unsorted, overlapping or repeated; each library call takes a group of them whose staging and output stay
-        bounded. Raises the first failing range's error."""
+        bounded. Raises the first failing range's error. With host streams this is the gather, split."""
+        if self._host:
+            return _split(*self.gather(ranges))
         ranges = [(int(i), int(lo), int(n)) for i, lo, n in ranges]
         for i, lo, n in ranges:
             if not 0 <= i < len(self._ins):

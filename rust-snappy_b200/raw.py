@@ -204,6 +204,52 @@ def _stored_tables(tables, lens, dev, magic, rec, records):
 
 
 GATHER_RANGES_PER_CALL = 1 << 20            # ranges one gather call takes: its scratch is 108 bytes each plus 256 MiB
+HOST_BUILD_BYTES = 1 << 30                  # compressed bytes a host-stream reader holds on the device to build tables
+
+
+def _host_streams(streams):
+    """The streams of a reader with host=True, as CPU uint8 tensors the device reads at their own addresses: bytes-like
+    streams copied once into one pinned buffer, pinned 1-D contiguous CPU uint8 tensors as they are. Anything else
+    raises ValueError before the library sees it; then every stream must pass sb_host_stream_check."""
+    import numpy as np
+    import torch
+    out, host = [], []
+    for i, s in enumerate(streams):
+        if isinstance(s, torch.Tensor):
+            if s.is_cuda or s.dtype != torch.uint8 or s.dim() != 1 or not s.is_contiguous() or not s.is_pinned():
+                raise ValueError("stream %d: host=True takes bytes-like streams or pinned contiguous 1-D CPU uint8 "
+                                 "tensors" % i)
+            out.append(s)
+        else:
+            host.append((i, np.frombuffer(s, dtype=np.uint8)))
+            out.append(None)
+    if host:                                                             # the bytes-like streams in one pinned copy
+        at = np.cumsum([0] + [v.size for _, v in host])
+        t_all = torch.empty(int(at[-1]) + 1, dtype=torch.uint8, pin_memory=True)
+        cat = t_all.numpy()
+        for (i, v), o in zip(host, at):
+            cat[o:o + v.size] = v
+            out[i] = t_all[int(o):int(o) + v.size]
+    L = _lib.lib()
+    for t in out:
+        e = _lib.SbError()
+        if L.sb_host_stream_check(t.data_ptr(), t.numel(), C.byref(e)):
+            raise from_c(e)
+    return out
+
+
+def _windows(which, lens, limit):
+    """Groups of `which` whose lengths sum to at most `limit`; a longer stream makes a group of its own."""
+    groups, cur, total = [], [], 0
+    for i in which:
+        if cur and total + lens[i] > limit:
+            groups.append(cur)
+            cur, total = [], 0
+        cur.append(i)
+        total += lens[i]
+    if cur:
+        groups.append(cur)
+    return groups
 
 
 def _check_ranges(ranges, count):
@@ -224,8 +270,9 @@ def _gather(reader, fmt, ranges, rooms, data, offs):
     import numpy as np
     import torch
     L = _lib.lib()
-    scratch_bytes = getattr(L, "sb_%s_table_gather_scratch_bytes" % fmt)
-    call = getattr(L, "sb_%s_table_gather_device_ws" % fmt)
+    kind = "gather_host_streams" if reader._host else "gather"
+    scratch_bytes = getattr(L, "sb_%s_table_%s_scratch_bytes" % (fmt, kind))
+    call = getattr(L, "sb_%s_table_%s%s" % (fmt, kind, "_ws" if reader._host else "_device_ws"))
     a, k = 0, len(ranges)
     rooms = np.asarray(rooms, dtype=np.int64)
     ends = np.cumsum(rooms)
@@ -257,6 +304,12 @@ def _gather(reader, fmt, ranges, rooms, data, offs):
     return None
 
 
+def _split(data, offs):
+    """What gather returned, as read_ranges returns it: one bytes object per range."""
+    back = data.cpu().numpy()
+    return [back[int(a):int(b)].tobytes() for a, b in zip(offs[:-1], offs[1:])]
+
+
 def _gathered(rooms):
     """The offsets of ranges packed back to back: len(rooms) + 1 int64 entries."""
     import numpy as np
@@ -278,19 +331,25 @@ class TableReader:
     tables: the streams' stored seek tables (from compress_batch(..., tables=True) or an earlier build), bytes-like or
     CUDA uint8 tensors, instead of a build. They are uploaded in one copy and no build runs; a table whose header does
     not match its stream's length raises ValueError. A table of another stream of the same length gives every read over
-    it that block's checksum error, never wrong bytes."""
+    it that block's checksum error, never wrong bytes.
+    host: the streams stay in pinned host memory (bytes-like ones copied once into one pinned buffer, pinned CPU uint8
+    tensors kept alive; unpinned CPU and CUDA tensors raise ValueError), so a corpus larger than the device can be read.
+    Only the tables live on the device: they are built from uploads of at most HOST_BUILD_BYTES of streams at a time.
+    Reads go through sb_raw_table_gather_host_streams_ws, which copies over PCIe only the compressed blocks it decodes;
+    read_ranges is then the gather, split. Results and errors are those of a reader without host."""
 
     RANGES_PER_CALL = 4096                    # 128 KiB of staging per range: 512 MiB per call at most
     BYTES_PER_CALL = 1 << 30                  # output bytes one call gathers (a single larger range gets its own call)
     GROUP_BYTES = 1 << 34                     # compressed bytes one build call takes (its scratch grows with them)
 
-    def __init__(self, streams, tables=None):
+    def __init__(self, streams, tables=None, host=False):
         import numpy as np
         import torch
         self._dev = torch.device("cuda", torch.cuda.current_device())
         self._cuda = torch.cuda.current_stream(self._dev).cuda_stream
-        self._ins, host = [], []
-        for s in streams:
+        self._host = bool(host)
+        self._ins, host = ([], []) if not self._host else (_host_streams(streams), [])
+        for s in streams if not self._host else ():
             if isinstance(s, torch.Tensor):
                 if not s.is_cuda or s.dtype != torch.uint8 or s.dim() != 1 or not s.is_contiguous():
                     raise ValueError("TableReader takes contiguous 1-D CUDA uint8 tensors")
@@ -323,8 +382,12 @@ class TableReader:
             self.lengths = [int(w[2]) if ok else None for w, ok in zip(heads, self.seekable)]
         else:
             ptrs, results = [0] * count, [None] * count
-            for i, p, r in self._build(list(range(count))):
-                ptrs[i], results[i] = p, r
+            groups = _windows(range(count), lens, HOST_BUILD_BYTES) if self._host else [list(range(count))]
+            for g in groups:                                             # host streams: one uploaded window at a time
+                ins = {i: self._ins[i].to(self._dev) for i in g} if self._host else self._ins
+                for i, p, r in self._build(g, ins):
+                    ptrs[i], results[i] = p, r
+                del ins
             self.seekable = [r.status.code == 0 for r in results]
             self.lengths = [int(r.bytes) if ok else None for r, ok in zip(results, self.seekable)]
         to64 = lambda v: torch.from_numpy(np.array(v, dtype=np.uint64).view(np.int64)).to(self._dev)
@@ -332,27 +395,18 @@ class TableReader:
         self._t_ins = to64([t.data_ptr() for t in self._ins] + [0])
         self._t_lens = to64(lens + [0])
 
-    def _build(self, which):
-        """sb_raw_table_build_batch_device_ws over groups of at most GROUP_BYTES compressed bytes: one call and one wait
-        per group. A group's tables stay in one buffer cut to their packed size. Yields (stream, its table's address, its
-        result) for every stream."""
+    def _build(self, which, streams):
+        """sb_raw_table_build_batch_device_ws over groups of at most GROUP_BYTES compressed bytes of `streams` (device
+        tensors by stream index): one call and one wait per group. A group's tables stay in one buffer cut to their
+        packed size. Yields (stream, its table's address, its result) for every stream."""
         import numpy as np
         import torch
         L = _lib.lib()
-        groups, cur, total = [], [], 0
-        for i in which:
-            n = self._ins[i].numel()
-            if cur and total + n > self.GROUP_BYTES:
-                groups.append(cur)
-                cur, total = [], 0
-            cur.append(i)
-            total += n
-        if cur:
-            groups.append(cur)
+        groups = _windows(which, [t.numel() if t is not None else 0 for t in self._ins], self.GROUP_BYTES)
         rsz = C.sizeof(_lib.SbFrameResult)
         for g in groups:
             k = len(g)
-            ins = [self._ins[i] for i in g]
+            ins = [streams[i] for i in g]
             in_bytes = sum(t.numel() for t in ins)
             desc = np.concatenate([np.array([t.data_ptr() for t in ins], dtype=np.uint64).view(np.int64),
                                    np.array([t.numel() for t in ins] + [0] * (k % 2), dtype=np.uint32).view(np.int64)])
@@ -427,7 +481,7 @@ class TableReader:
         at = np.zeros(k, dtype=np.int64)
         at[1:] = np.cumsum(caps[:-1])
         t_out = torch.empty(sum(caps) + 1, dtype=torch.uint8, device=self._dev)
-        ins = [self._ins[i] for i, _ in todo]
+        ins = [self._ins[i].to(self._dev) for i, _ in todo]                # host streams: uploaded for this call
         desc = np.concatenate([np.array([t.data_ptr() for t in ins], dtype=np.uint64).view(np.int64), at + t_out.data_ptr(),
                                np.array([t.numel() for t in ins] + caps, dtype=np.uint32).view(np.int64)])
         t_desc = torch.from_numpy(desc).to(self._dev)
@@ -457,7 +511,9 @@ class TableReader:
     def read_ranges(self, ranges) -> list:
         """One bytes object per (i, lo, n) range of stream i. Ranges may mix streams in any order and be empty,
         unsorted, overlapping or repeated; each library call takes a group of them whose staging and output stay
-        bounded. Raises the first failing range's error."""
+        bounded. Raises the first failing range's error. With host streams this is the gather, split."""
+        if self._host:
+            return _split(*self.gather(ranges))
         ranges = [(int(i), int(lo), int(n)) for i, lo, n in ranges]
         for i, lo, n in ranges:
             if not 0 <= i < len(self._ins):
