@@ -60,7 +60,32 @@ SB_DEVICE uint32_t k2_decode_stream(const uint8_t* in, uint32_t n, uint8_t* dst,
     const uint32_t sn = n - hl, dn = (uint32_t)dn64;        // both < 2^32 (checked above)
     uint32_t s = 0, d = 0;
 
+    // Input words kept across windows: lane i holds the 4 bytes at src + wb + 4i, an aligned 128-byte span (bytes outside
+    // [in, in_end) read as zero). A window needs the 36 bytes from s on, which a span holds while s - wb <= 92; a window
+    // advances by about 32 to 40 bytes, so on text the span is refilled about every third window, and after every spill.
+    uint32_t word = 0, wb = 0u - 128u;                       // the first window refills
     while (s < sn) {
+        uint32_t lo, hi;
+        unsigned sh;
+        {
+            if (s - wb > 92u) {
+                const uintptr_t A = (uintptr_t)(src + s);
+                const unsigned mis = (unsigned)(A & 3u);
+                wb = s - mis;
+                const uint8_t* wp = (const uint8_t*)(A - mis) + 4 * lane;
+                if (wp >= in && wp + 4 <= in_end) {
+                    word = *(const uint32_t*)wp;
+                } else {
+                    word = 0;
+                    for (int k = 0; k < 4; k++)
+                        if (wp + k >= in && wp + k < in_end) word |= (uint32_t)wp[k] << (8 * k);
+                }
+            }
+            const unsigned bi = s - wb + lane;
+            lo = shfl(word, bi >> 2);
+            hi = shfl(word, (bi >> 2) + 1);
+            sh = (bi & 3u) * 8;
+        }
 #include "k2_window.inc"
         const bool is_start = ((M >> lane) & 1u) && valid;
         const unsigned last = 31 - clz(M);

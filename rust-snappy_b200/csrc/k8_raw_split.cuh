@@ -132,6 +132,27 @@ SB_DEVICE uint64_t k8_walk(const RawPlan& p, uint64_t s0, uint64_t stop, uint64_
     uint32_t s = (uint32_t)s0, piece = s;                            // piece: where the current canonical parse began
     uint64_t d = 0;
     while (s < stop) {
+        // the window's 40 bytes from the aligned word at or before src + s, fetched per window: a restart moves s back
+        uint32_t lo, hi;
+        unsigned sh;
+        {
+            const uintptr_t A = (uintptr_t)(src + s);
+            const unsigned mis = (unsigned)(A & 3u);
+            uint32_t word = 0;
+            if (lane < 10) {
+                const uint8_t* wp = (const uint8_t*)(A - mis) + 4 * lane;
+                if (wp >= in && wp + 4 <= in_end) {
+                    word = *(const uint32_t*)wp;
+                } else {
+                    for (int k = 0; k < 4; k++)
+                        if (wp + k >= in && wp + k < in_end) word |= (uint32_t)wp[k] << (8 * k);
+                }
+            }
+            const unsigned bi = mis + lane;
+            lo = shfl(word, bi >> 2);
+            hi = shfl(word, (bi >> 2) + 1);
+            sh = (bi & 3u) * 8;
+        }
 #include "k2_window.inc"
         (void)off; (void)spill; (void)E; (void)valid;
         const uint64_t lim = stop - s;                                  // <= rem

@@ -175,7 +175,11 @@ __global__ void __launch_bounds__(128, 8) k18_raw_gather_kernel(sbk::GatherPlan<
 
 std::atomic<uint64_t> g_launches{0};
 std::atomic<uint64_t> g_allocs{0};     // cudaMalloc / cudaHostAlloc / event + stream creations since load
-const int K2_DEFAULT_CTAS_PER_SM = 16;
+// K2: 0 = one warp per unit, and the hardware hands out CTAs as residents finish. With a capped grid every warp strides
+// over a fixed share of units, and the CTAs beyond the resident ones start late and end the launch at low occupancy
+// (DESIGN.md section 5: 104 -> 120 GB/s on the bench's 131,072-unit waves). SNAPB200_K2_CTAS caps the grid per SM.
+const int K2_DEFAULT_CTAS_PER_SM = 0;
+const int K8B_FINISH_CTAS_PER_SM = 16;
 // H100 (50 MB L2): the 7 shared-memory chains per SM already keep more input windows hot than L2 holds, and every
 // L2-table chain adds its table and window on top; 7 + 0 chains measured fastest (DESIGN.md section 5)
 const int K1_DEFAULT_NG = 0;
@@ -341,11 +345,10 @@ int launch_k2(Ctx& c, const sb_batch& b, cudaStream_t st, sb_error* err) {
     if (b.count == 0) return 0;
     const unsigned wpb = 4;
     uint64_t blocks = ((uint64_t)b.count + wpb - 1) / wpb;
-    // resident CTAs per SM: each warp keeps a 64KB output history alive, and copy sources are
-    // re-read from it -- too many streams in flight and the history falls out of the 50MB L2
+    // the grid does not set how many streams are in flight: registers fix the resident CTAs per SM (10 at 48 registers)
     static const int per_sm = getenv("SNAPB200_K2_CTAS") ? atoi(getenv("SNAPB200_K2_CTAS")) : K2_DEFAULT_CTAS_PER_SM;
-    unsigned grid = (unsigned)(per_sm * c.sms);
-    if (grid > blocks) grid = (unsigned)blocks;
+    uint64_t cap = per_sm > 0 ? (uint64_t)per_sm * c.sms : (uint64_t)INT32_MAX;   // the kernel strides past the grid
+    const unsigned grid = (unsigned)(blocks < cap ? blocks : cap);
     k2_decompress_kernel<<<grid, 32 * wpb, wpb * sbk::K2_SMEM_PER_WARP, st>>>(b);
     g_launches++;
     CK(cudaGetLastError());
@@ -642,7 +645,7 @@ int launch_raw_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_u
     // the payload part: warps over the block list, whose true length is on the device, then the one-warp pass, sized
     // like launch_k2
     k8b_blocks_kernel<<<device_grid(c, q.in_bytes / 3072 + b.count, 4, 16), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
-    static const int per_sm = getenv("SNAPB200_K2_CTAS") ? atoi(getenv("SNAPB200_K2_CTAS")) : K2_DEFAULT_CTAS_PER_SM;
+    static const int per_sm = getenv("SNAPB200_K2_CTAS") ? atoi(getenv("SNAPB200_K2_CTAS")) : K8B_FINISH_CTAS_PER_SM;
     k8b_finish_kernel<<<device_grid(c, b.count, 4, per_sm), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
     g_launches += 2;
     CK(cudaGetLastError());

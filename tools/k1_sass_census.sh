@@ -18,33 +18,39 @@
 # across the back edge into the next iteration. A wait a few instructions after a long-latency load is a stall.
 # usage: tools/k1_sass_census.sh [extra nvcc flags, e.g. -DK1_PROFILE]
 #   NG=5|7 picks the kernel, MIN=n hides loops under n instructions, SASS=1 reuses the listing already in $OUT
+#   KERNEL=<mangled-name fragment> and DEPTH=n census another kernel and default WAITS to its largest loop at depth n
+#   (tools/k2_sass_census.sh does so for K2)
 # The cubin, the SASS listing and the ptxas log go to $OUT (default build/k1_exp, kept out of git).
 set -e
 cd "$(dirname "$0")/.."
 OUT=${OUT:-build/k1_exp}
 NG=${NG:-0}
 MIN=${MIN:-40}     # loops shorter than this many instructions are not listed
+KERNEL=${KERNEL:-k1_m7_kernelILi${NG}E}
+DEPTH=${DEPTH:-2}
 mkdir -p "$OUT"
 [ -n "$SASS" ] || nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xptxas -v "$@" -cubin \
      -o "$OUT/census.cubin" rust-snappy_b200/csrc/snapb200.cu 2> "$OUT/census.ptxas.log"
 [ -n "$SASS" ] || cuobjdump -sass "$OUT/census.cubin" > "$OUT/census.sass"
-python3 - "$OUT/census.sass" "$OUT/census.ptxas.log" "$NG" "$MIN" "${WAITS:-0}" "${HEAD:-}" "$OUT/census.ctrl" <<'PY'
+python3 - "$OUT/census.sass" "$OUT/census.ptxas.log" "$KERNEL" "$MIN" "${WAITS:-0}" "${HEAD:-}" "$OUT/census.ctrl" "$DEPTH" <<'PY'
 import re, sys
-sass, log, ng, minlen = sys.argv[1], sys.argv[2], sys.argv[3], int(sys.argv[4])
-waits, head_arg, ctrl_out = sys.argv[5] == "1", sys.argv[6], sys.argv[7]
-# registers and spills of every K1 kernel
+sass, log, kname, minlen = sys.argv[1], sys.argv[2], sys.argv[3], int(sys.argv[4])
+waits, head_arg, ctrl_out, wdepth = sys.argv[5] == "1", sys.argv[6], sys.argv[7], int(sys.argv[8])
+# registers and spills of every kernel of the same family (k1_m7_kernel<NG> for K1)
+family = re.sub(r"ILi\d+E$", "", kname)
+show = lambda name: re.sub(r"ILi(\d+)E?$", r"<\1>", name)      # k1_m7_kernelILi0E -> k1_m7_kernel<0>
 lines = open(log).read().splitlines()
 for i, l in enumerate(lines):
-    m = re.search(r"Compiling entry function '\w*k1_m7_kernelILi(\d+)E\w*'", l)
+    m = re.search(r"Compiling entry function '\w*?(%s\w*?)(E\w*)?'" % re.escape(family), l)
     if m:
         info = " ".join(x.split(":", 1)[-1].strip() for x in lines[i + 1:i + 4] if "bytes stack" in x or "Used" in x)
-        print("k1_m7_kernel<%s>: %s" % (m.group(1), info))
+        print("%s: %s" % (show(m.group(1)), info))
 # instructions of k1_m7_kernel<NG>: [address, opcode, branch target or None, predicated, text]; hi[k] = high
 # 64 bits of the encoding, which cuobjdump prints alone on the line after the instruction; raw[k] = text with predicate
 ins, hi, raw, on = [], [], [], False
 for l in open(sass):
     if "Function :" in l:
-        on = ("k1_m7_kernelILi%sE" % ng) in l
+        on = kname in l
         continue
     if not on:
         continue
@@ -62,8 +68,8 @@ for l in open(sass):
     t = re.search(r"\b0x([0-9a-f]+)\s*$", text)
     ins.append((int(m.group(1), 16), op, int(t.group(1), 16) if t else None, pred, text))
 if not ins:
-    sys.exit("k1_m7_kernel<%s> not found in %s" % (ng, sass))
-print("k1_m7_kernel<%s>: %d SASS instructions" % (ng, sum(1 for a in ins if a[1] != "NOP")))
+    sys.exit("%s not found in %s" % (kname, sass))
+print("%s: %d SASS instructions" % (show(kname), sum(1 for a in ins if a[1] != "NOP")))
 # control-flow graph over instructions. BSYNC Bx continues at the target the last BSSY Bx on the way set: the possible
 # targets per barrier register are propagated forward along the edges until nothing changes.
 idx = {a[0]: k for k, a in enumerate(ins)}
@@ -138,7 +144,7 @@ def ctrl(k):
 if head_arg:
     h0 = idx[int(head_arg, 16)]
 else:
-    depth2 = [h for h in loops if sum(1 for h2 in loops if h2 != h and loops[h] < loops[h2]) == 2]
+    depth2 = [h for h in loops if sum(1 for h2 in loops if h2 != h and loops[h] < loops[h2]) == wdepth]
     h0 = max(depth2, key=lambda h: len(loops[h]))
 body = loops[h0]
 order = sorted(body)
