@@ -12,16 +12,16 @@
 // memory / L2, with its 16K-entry u16 hash table in shared memory (7 chains) or in
 // an L2-resident global scratch (the others):
 //
-//  * PARSER warp. Looks at 32 consecutive positions at once. Every lane hashes
-//    its position, reads the table as of the window start, fetches its
-//    candidate and computes "would a probe here hit, and how long is the match".
-//    From the hit bitmask each hit lane computes where the NEXT copy would start
+//  * PARSER warp. Looks at 64 consecutive positions per step, two per lane. Every
+//    lane hashes its positions, reads the table as of the step start, fetches the
+//    candidates and computes "would a probe here hit, and how long is the match".
+//    From the hit bitmask each hit position computes where the NEXT copy would start
 //    (rematch hit at the copy end, else the first later hit of the scan), pointer
-//    doubling from the window's entry state yields the copies the serial encoder
+//    doubling from the step's entry state yields the copies the serial encoder
 //    takes, and the inserted positions are "everything except copy interiors".
-//    The inserts are committed; if two inserted lanes collided on a slot, the
-//    window is accepted up to the first lane whose candidate should have come from
-//    inside the window and restarts there.
+//    The inserts are committed; if two inserted positions collided on a slot, the
+//    step is accepted up to the first position whose candidate should have come from
+//    inside the step and restarts there.
 //  * serial path: the reference's control flow executed by the warp (scan probes
 //    32 at a time with match.any conflict resolution, 128-byte match extension).
 //    Used for scan runs past 32 probes (stride > 1) and the block tail.
@@ -29,9 +29,9 @@
 //    from a ring, 32 at a time: literal/copy tag sizes, a warp scan for output
 //    offsets, tags and literal bytes written straight to HBM (evict-first).
 //
-// Tried and rejected (slower on hardware): 64-position steps, unaligned windows, speculative slot reads for the
-// L2-table chains, an mbarrier wake-up for the emitter, and a second-generation parser with exact windows and
-// pipelined candidate evaluation. The one-pair-per-CTA layouts of round 1 (shared-memory window, pipelined parser
+// Tried and rejected (slower on hardware): 32-position steps, unaligned windows,
+// speculative slot reads for the L2-table chains, an mbarrier wake-up for the emitter, and a second-generation parser
+// with exact windows and pipelined candidate evaluation. The one-pair-per-CTA layouts of round 1 (shared-memory window, pipelined parser
 // warps) are gone as well (DESIGN.md section 4).
 #pragma once
 #include "common.cuh"
@@ -40,7 +40,7 @@
 #if defined(K1_PROFILE) && defined(__CUDACC__)
 // Optional phase timers for kernel archaeology (tools/k1_phase_profile.sh builds a separate
 // library with -DK1_PROFILE; the product build has none of this).
-// [0..11]: cycles per phase (K1_TICK slots), [12 + s]: parser warps per scheduler, [16 + k]: K1_COUNT(k) windows
+// [0..11]: cycles per phase (K1_TICK slots), [12 + s]: parser warps per scheduler, [16 + k]: K1_COUNT(k) steps
 __device__ unsigned long long g_k1_prof[18];
 #define K1_TICK(slot) do { const long long _now = clock64(); if (sbk::lane_id() == 0) k1_acc[slot] += (unsigned long long)(_now - k1_t0); k1_t0 = _now; } while (0)
 #define K1_COUNT(k) do { if (sbk::lane_id() == 0) k1_acc[12 + (k)]++; } while (0)
@@ -59,16 +59,16 @@ __device__ unsigned long long g_k1_prof[18];
 #define K1_PROF_PASS
 #define K1_PROF_FLUSH do { } while (0)
 #if defined(SB_EMU)
-// CPU warp-emulator build (tests/emu): the same window counts, readable by the tests through the symbol
+// CPU warp-emulator build (tests/emu): the same step counts, readable by the tests through the symbol
 extern "C" { __attribute__((weak)) unsigned long long sb_emu_k1_windows[4]; }
 #define K1_COUNT(k) do { if (sbk::lane_id() == 0) sb_emu_k1_windows[k]++; } while (0)
 #else
 #define K1_COUNT(k) do { } while (0)
 #endif
 #endif
-// K1_COUNT: [0] fast-path windows whose probe the previous window issued (hoisted), [1] probes issued at the loop top;
-// emulator build only: [2] probes whose table slot changed between the read and the use, [3] sequential-word fetches
-// that reach byte n of the block (both must stay 0)
+// K1_COUNT: [0] fast-path steps whose probe the previous step issued (hoisted), [1] probes issued at the loop top;
+// emulator build only: [2] probes with a table slot that changed between the read and the use, [3] sequential-word
+// fetches that reach byte n of the block (both must stay 0)
 
 namespace sbk {
 
@@ -104,7 +104,7 @@ SB_DEVICE uint64_t k1_event(uint32_t pos, uint32_t len, uint32_t off) {
 // producer side. The parser keeps private copies of the ring counters and only
 // touches the shared ones when it has to: `tail_seen` is refreshed when the ring
 // looks full, `head` is published every K1_PUBLISH events (the emitter works on
-// fuller batches and the parser pays one fence per batch instead of one per window).
+// fuller batches and the parser pays one fence per batch instead of one per step).
 struct K1Prod {
     uint32_t head;        // events written so far
     uint32_t published;   // value of ctrl[0]
@@ -162,10 +162,10 @@ struct K1State {
     uint32_t skip;     // scan state (src/compress.rs:204-211); meaningful when !rematch
     bool rematch;      // true: a copy just ended at s and s-1 is already inserted (:285-301 first half)
 };
-// the window at w (holding st.s) runs on the parser's fast path: well inside the block, and a scan still probes
-// every position
+// the step at w (holding st.s) runs on the parser's fast path: well inside the block (every position up to w + 63
+// may be probed, and the words it reads end before byte n), and a scan still probes every position
 SB_DEVICE bool k1_fast(uint32_t w, const K1State& st, uint32_t s_limit) {
-    return w + 36 < s_limit && (st.rematch || st.skip < 64);
+    return w + 68 < s_limit && (st.rematch || st.skip < 64);
 }
 
 #define K1_HASH(x) (((uint32_t)(x) * 0x1E35A7BDu) >> shift)
@@ -248,19 +248,9 @@ SB_DEVICE bool k1_serial(const uint8_t* win, uint32_t n, uint16_t* table, unsign
     }
 }
 
-// Per-lane result of probing one 32-position window against the table as it was when
-// the probe ran (possibly a little stale when several parser warps are pipelined).
-struct K1Pre {
-    uint32_t h;      // hash of this lane's position
-    uint32_t c;      // candidate read from the table
-    uint32_t L;      // match length: exact up to 15, 16 = "16 or more"
-    uint32_t E;      // ballot: a probe at lane i would hit
-    uint32_t M;      // copy starts reachable from this lane (pointer doubling), valid if !(M & longs)
-    uint32_t longs;  // ballot: hit whose length is only known to be >= 16
-    bool eq;
-};
-// the four sequential words a lane needs for a window, fetched one window ahead when the
-// window lives in global memory (hides one L2 round trip per window)
+// A step covers the 64 positions [w, w + 64) with w = s & ~31: lane l owns position w + l (half 0) and w + 32 + l
+// (half 1). The sequential words a lane needs for one half, fetched one step ahead when the block lives in global
+// memory (hides one L2 round trip per step)
 struct K1Seq { uint32_t a0, a1, a2, a3, a4, w; };
 SB_DEVICE K1Seq k1_fetch_seq(const uint8_t* win, uint32_t w, uint32_t n) {
     const uintptr_t aa = (uintptr_t)(win + w + lane_id());
@@ -275,26 +265,7 @@ SB_DEVICE K1Seq k1_fetch_seq(const uint8_t* win, uint32_t w, uint32_t n) {
     return q;
 }
 
-// "next copy start" pointer doubling over the hit lanes of a window
-SB_DEVICE uint32_t k1_double(uint32_t E, bool eq, uint32_t L) {
-    const unsigned lane = lane_id();
-    const uint32_t e = lane + L;
-    // next copy start after a copy ending at e: a rematch hit at e itself, else the first later hit
-    // of the scan -- i.e. simply the first hit at or after e
-    uint32_t T = 64;
-    if (eq && e < 32) { const uint32_t m = E >> e; if (m) T = e + (uint32_t)(ffs(m) - 1); }
-    // copies are >= 4 bytes long and do not overlap, so a 32-position window holds at most 8 copy
-    // starts on any chain: three doubling rounds (2^3 nodes) always reach the end of the chain
-    uint32_t M = 1u << lane;
-#pragma unroll
-    for (int r = 0; r < 3; r++) {
-        const uint32_t M2 = shfl(M, T & 31u), T2 = shfl(T, T & 31u);
-        if (T < 32) { M |= M2; T = T2; }
-    }
-    return M;
-}
-
-// A window's probe between its issue and its use: the lane's hash, the table slot and the
+// A half's probe between its issue and its use: the lane's hash, the table slot and the
 // candidate's five aligned words, whose loads may still be in flight.
 struct K1Probe { uint32_t h, c, b0, b1, b2, b3, b4; };
 SB_DEVICE K1Probe k1_probe_issue(const uint8_t* win, const uint16_t* table, unsigned shift, const K1Seq& q) {
@@ -306,17 +277,23 @@ SB_DEVICE K1Probe k1_probe_issue(const uint8_t* win, const uint16_t* table, unsi
     r.b0 = bw[0]; r.b1 = bw[1]; r.b2 = bw[2]; r.b3 = bw[3]; r.b4 = bw[4];
     return r;
 }
-// compare, match length, hit ballots and pointer doubling of a probe issued on the words `q`
-SB_DEVICE K1Pre k1_probe_complete(const uint8_t* win, const K1Seq& q, const K1Probe& pb) {
+
+// one position probed against the table as it was when the probe was issued
+struct K1Hit {
+    uint32_t h;      // hash of the position
+    uint32_t c;      // candidate read from the table
+    uint32_t L;      // match length: exact up to 15, 16 = "16 or more"
+    bool eq;         // a probe here would hit
+};
+SB_DEVICE K1Hit k1_probe_match(const uint8_t* win, const K1Seq& q, const K1Probe& pb) {
     const unsigned ash = (unsigned)((uintptr_t)(win + q.w + lane_id()) & 3u) * 8;
     const uint32_t a0 = q.a0, a1 = q.a1, a2 = q.a2, a3 = q.a3, a4 = q.a4;
     const uint32_t b0 = pb.b0, b1 = pb.b1, b2 = pb.b2, b3 = pb.b3, b4 = pb.b4;
     const unsigned bsh = (unsigned)((uintptr_t)(win + pb.c) & 3u) * 8;
-    const uint32_t cur = funnel_r(a0, a1, ash);
-    K1Pre r;
+    K1Hit r;
     r.h = pb.h;
     r.c = pb.c;
-    r.eq = cur == funnel_r(b0, b1, bsh);
+    r.eq = funnel_r(a0, a1, ash) == funnel_r(b0, b1, bsh);
     // match length, branch-free: bytes 4..15 of both sides, first differing byte wins
     {
         const uint32_t x4 = funnel_r(a1, a2, ash) ^ funnel_r(b1, b2, bsh);
@@ -327,100 +304,181 @@ SB_DEVICE K1Pre k1_probe_complete(const uint8_t* win, const K1Seq& q, const K1Pr
         const uint32_t lb = x4 ? 4u : x8 ? 8u : 12u;
         r.L = x ? lb + ((uint32_t)(ffs(x) - 1) >> 3) : 16;
     }
-    r.E = ballot(r.eq);
-    r.longs = ballot(r.eq && r.L == 16);
-    r.M = k1_double(r.E, r.eq, r.L);
     return r;
 }
 
-// Finish one window from a probe result that is known to be current for every lane
+// "Next copy start" pointer doubling over the step's 64 positions. Node x's successor is the first hit at or after
+// the end x + L of its copy (a rematch hit at the end itself, else the first later hit of the scan), 64 for none.
+// Successors lie after their node, so a half-1 node's chain stays in half 1: each half doubles on its own, and a
+// half-0 chain records where it leaves half 0. Copies are >= 4 bytes long and do not overlap, so a chain holds at most
+// 8 copy starts in a half: three rounds (2^3 nodes) always reach its end.
+struct K1Chains {
+    uint32_t M0;     // half-0 copy starts reachable from the lane's half-0 node
+    uint32_t X0;     // first node at or past 32 that chain reaches (64: none)
+    uint32_t M1;     // half-1 copy starts reachable from the lane's half-1 node (bit i: position 32 + i)
+    uint32_t bad;    // ballot: after the copy of the half-0 node, the scan leaves stride 1 inside the step
+};
+SB_DEVICE K1Chains k1_double(uint64_t E, bool eq0, uint32_t L0, bool eq1, uint32_t L1) {
+    const unsigned lane = lane_id();
+    const uint32_t e0 = lane + L0, e1 = 32 + lane + L1;
+    uint32_t T0 = 64, T1 = 64;
+    if (eq0 && e0 < 64) { const uint64_t m = E >> e0; if (m) T0 = e0 + (uint32_t)(ffsll(m) - 1); }
+    if (eq1 && e1 < 64) { const uint64_t m = E >> e1; if (m) T1 = e1 + (uint32_t)(ffsll(m) - 1); }
+    K1Chains r;
+    // a rematch miss at e0 starts a scan at e0 + 1 with skip 32; it probes up to the next copy start or the end of
+    // the step, and more than 32 such probes would leave stride 1 (a half-1 copy ends at 36 or later: never)
+    r.bad = ballot(eq0 && (T0 < 64 ? T0 : 63u) > e0 + 32);
+    uint32_t M0 = 1u << lane, M1 = 1u << lane;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const uint32_t M0n = shfl(M0, T0 & 31u), T0n = shfl(T0, T0 & 31u);
+        const uint32_t M1n = shfl(M1, T1 & 31u), T1n = shfl(T1, T1 & 31u);
+        if (T0 < 32) { M0 |= M0n; T0 = T0n; }
+        if (T1 < 64) { M1 |= M1n; T1 = T1n; }
+    }
+    r.M0 = M0; r.X0 = T0; r.M1 = M1;
+    return r;
+}
+
+// a step's two halves after the compare: hits, hit ballots over the 64 positions and the doubled chains
+struct K1Pre {
+    K1Hit x0, x1;
+    uint64_t E;      // a probe at position i would hit
+    uint64_t longs;  // hit whose length is only known to be >= 16
+    K1Chains ch;
+};
+SB_DEVICE K1Pre k1_probe_complete(const uint8_t* win, const K1Seq* q, const K1Probe* pb) {
+    K1Pre r;
+    r.x0 = k1_probe_match(win, q[0], pb[0]);
+    r.x1 = k1_probe_match(win, q[1], pb[1]);
+    r.E = ballot(r.x0.eq) | (uint64_t)ballot(r.x1.eq) << 32;
+    r.longs = ballot(r.x0.eq && r.x0.L == 16) | (uint64_t)ballot(r.x1.eq && r.x1.L == 16) << 32;
+    r.ch = k1_double(r.E, r.x0.eq, r.x0.L, r.x1.eq, r.x1.L);
+    return r;
+}
+
+// positions [x + 1, x + L - 2] of a copy at x (L >= 4), clipped to the step: not inserted; branch-free
+SB_DEVICE uint64_t k1_interior(uint32_t x, uint32_t L) {
+    const uint32_t hi = x + L - 2;
+    const uint64_t upto = hi >= 63 ? ~0ull : ((2ull << hi) - 1ull);
+    return upto & ~((2ull << x) - 1ull);                          // (2 << 63) wraps to 0: position 63 has no interior
+}
+
+// the step's copies to the ring in position order; slot0 / slot1: a lane's event among them for each half
+SB_DEVICE void k1_push_copies(const K1Ring& r, K1Prod& pr, uint32_t ncopy, bool taken0, uint32_t slot0, uint64_t ev0,
+                              bool taken1, uint32_t slot1, uint64_t ev1) {
+    if (!ncopy) return;
+    k1_wait_space(r, pr, ncopy);
+    if (taken0) r.ev[(pr.head + slot0) & (r.size - 1)] = ev0;
+    if (taken1) r.ev[(pr.head + slot1) & (r.size - 1)] = ev1;
+    pr.head += ncopy;
+    if (pr.head - pr.published >= K1_PUBLISH) k1_publish(r, pr);
+}
+
+// Finish one step from a probe result that is known to be current for every lane
 // from the entry position on. Returns false (state untouched, table restored) when
-// the window must be replayed serially. `nxt` holds the sequential words prefetched for w + 32;
-// `hoisted` tells whether the next window's probe was issued into `nextp` (DESIGN.md section 4).
-// GT: the table lives in global memory (L2) instead of shared memory -- a re-read costs a
-// full L2 round trip there, so slot clashes are found by comparing hashes across lanes.
-template <bool GT>
+// the step must be replayed serially. `nxt` holds the sequential words prefetched for w + 64 and w + 96;
+// `hoisted` tells whether the next step's probe was issued into `nextp` (DESIGN.md section 4).
 SB_DEVICE bool k1_finish(const uint8_t* win, uint32_t n, uint16_t* table, unsigned shift, uint32_t s_limit,
                          K1State& st, const K1Ring& ring, K1Prod& head, const K1Pre& pre, const K1Seq* nxt,
-                         K1Probe& nextp, bool& hoisted K1_PROF_ARGS) {
+                         K1Probe* nextp, bool& hoisted K1_PROF_ARGS) {
     const unsigned lane = lane_id();
     hoisted = false;
-    const uint32_t w = st.s & ~31u, i0 = st.s - w, p = w + lane;
-    const uint32_t h = pre.h, c = pre.c, E = pre.E;
-    const bool eq = pre.eq;
-    uint32_t L = pre.L;
-    // first copy start from the entry state
-    const uint32_t fm = E >> i0;                                 // i0 < 32
-    const uint32_t f = fm ? i0 + (uint32_t)(ffs(fm) - 1) : 32;   // rematch probe at i0 or scan from i0: first hit at/after i0
-    if (!st.rematch) {
-        const uint32_t probes = f < 32 ? f - i0 + 1 : 32 - i0;
-        if (st.skip + probes > 64) return false;                 // the run leaves stride 1 inside this window
-    }
-    // ---- which hits are taken: the probe's pointer doubling, redone only when a taken
-    // copy's length is not exact yet (>= 12): that copy is extended cooperatively first
-    uint32_t longmask = pre.longs, M = pre.M, CS;   // CS: lanes whose hit is taken as a copy
+    const uint32_t w = st.s & ~31u, i0 = st.s - w, p0 = w + lane, p1 = p0 + 32;
+    const uint32_t h0 = pre.x0.h, c0 = pre.x0.c, h1 = pre.x1.h, c1 = pre.x1.c;
+    const uint64_t E = pre.E;
+    uint32_t L0 = pre.x0.L, L1 = pre.x1.L;
+    // first copy start from the entry state: a rematch probe at i0 or a scan from i0, i.e. the first hit at/after i0
+    const uint64_t fm = E >> i0;                                 // i0 < 32
+    const uint32_t f = fm ? i0 + (uint32_t)(ffsll(fm) - 1) : 64;
+    // the scan up to it (or to the end of the step) stays at stride 1: after a rematch miss at i0 it probes i0 + 1..f
+    // with skip from 32, else i0..f with the running skip
+    if ((st.rematch ? 31u : st.skip) + (f < 64 ? f : 63u) - i0 >= 64) return false;
+    // ---- which hits are taken: the probe's pointer doubling, redone only when a taken copy's length is not exact
+    // yet (>= 16) and its end can fall inside the step: that copy is extended cooperatively first
+    uint64_t longmask = pre.longs;
+    K1Chains ch = pre.ch;
+    uint32_t CS0, CS1;                                           // taken copy starts: positions i, 32 + i
     for (;;) {
-        CS = f < 32 ? shfl(M, f) : 0;
-        const uint32_t unk = CS & longmask;
+        const uint32_t fs = f & 31u;
+        const uint32_t X0 = shfl(ch.X0, fs), M0 = shfl(ch.M0, fs);
+        const uint32_t X = f < 32 ? X0 : f;                      // the entry chain's first node in half 1
+        CS0 = f < 32 ? M0 : 0u;
+        CS1 = X < 64 ? shfl(ch.M1, X & 31u) : 0u;
+        const uint64_t unk = (CS0 | (uint64_t)CS1 << 32) & longmask;
         if (!unk) break;
-        const unsigned j = ffs(unk) - 1;
-        const uint32_t pj = w + j, cj = shfl(c, j);
+        const unsigned j = ffsll(unk) - 1;
+        const uint32_t pj = w + j, cj = shfl(j < 32 ? c0 : c1, j & 31u);
         const uint32_t end = k1_extend(win, n, pj + 16, cj + 16);
-        if (lane == j) L = end - pj;
-        longmask &= ~(1u << j);
-        M = k1_double(E, eq, L);
+        if (lane == (j & 31u)) { if (j < 32) L0 = end - pj; else L1 = end - pj; }
+        longmask &= ~(1ull << j);
+        // a copy from 48 on ends past the step whatever its length: its node keeps "no successor"
+        if (j < 48) ch = k1_double(E, pre.x0.eq, L0, pre.x1.eq, L1);
     }
+    if (CS0 & ch.bad) return false;                              // a scan after a taken copy leaves stride 1
     K1_TICK(3);                                                  // [3] entry state -> taken copies (+ long extensions)
-    // ---- inserted positions = entry..31 minus copy interiors [q+1, e-2]
-    const bool taken = (CS >> lane) & 1u;
-    // interior of my copy = lanes [lane+1, lane+L-2] (L >= 4), clipped to the window; branch-free
-    const uint32_t hi_ = lane + L - 2;
-    const uint32_t upto_ = hi_ >= 31 ? 0xFFFFFFFFu : ((2u << hi_) - 1u);
-    const uint32_t interior = taken ? (upto_ & ~((2u << lane) - 1u)) : 0u;   // (2<<31) wraps to 0: lane 31 has no interior
-    const uint32_t I = reduce_or(interior);
-    const uint32_t C = (0xFFFFFFFFu << i0) & ~I;
-    const bool ins = (C >> lane) & 1u;
+    // ---- inserted positions = entry..63 minus copy interiors [q+1, e-2]
+    const bool taken0 = (CS0 >> lane) & 1u, taken1 = (CS1 >> lane) & 1u;
+    const uint64_t interior = (taken0 ? k1_interior(lane, L0) : 0ull) | (taken1 ? k1_interior(32 + lane, L1) : 0ull);
+    const uint32_t C0 = (0xFFFFFFFFu << i0) & ~reduce_or((uint32_t)interior);
+    const uint32_t C1 = ~reduce_or((uint32_t)(interior >> 32));
+    const bool ins0 = (C0 >> lane) & 1u, ins1 = (C1 >> lane) & 1u;
 #ifdef SB_EMU_TRACE
-    if (lane == 0) fprintf(stderr, "win w=%u i0=%u rm=%d skip=%u E=%08x f=%u CS=%08x C=%08x\n", w, i0, (int)st.rematch, st.skip, E, f, CS, C);
+    if (lane == 0) fprintf(stderr, "step w=%u i0=%u rm=%d skip=%u E=%016llx f=%u CS=%08x%08x C=%08x%08x\n", w, i0,
+                           (int)st.rematch, st.skip, (unsigned long long)E, f, CS1, CS0, C1, C0);
 #endif
     K1_TICK(4);                                                  // [4] interiors / inserted mask
+    // the last writer of a slot wins: half 1 is stored after half 0, and within a half exactly one store lands
+    // (detected below)
     syncwarp();                                                  // every lane's probe read precedes the commit
-    if (ins) table[h] = (uint16_t)p;                             // same-slot stores: exactly one lands (detected below)
+    if (ins0) table[h0] = (uint16_t)p0;
     syncwarp();
-    uint32_t same = 0;
-    bool clash;
-    if (GT) { same = match_any(ins ? h : 0xFFFF0000u | lane); clash = ins && (same & (same - 1u)) != 0; }
-    else clash = ins && table[h] != (uint16_t)p;
-    uint32_t cut = 32;                                           // window accepted up to (not including) this lane
+    if (ins1) table[h1] = (uint16_t)p1;
+    syncwarp();
+    const bool clash = (ins0 && table[h0] != (uint16_t)p0) | (ins1 && table[h1] != (uint16_t)p1);
+    const uint32_t below = (1u << lane) - 1u, above = ~((2u << lane) - 1u);
     if (any(clash)) {
-        // Two inserted lanes share a slot. A probed lane with a lower inserted lane of the same
-        // hash should have seen that lane as its candidate ("victim"): everything before the
-        // first victim is still exactly what the serial encoder does, so keep that prefix and
-        // restart the window at the victim. Copy-end pre-inserts (e-1) are write-only, never victims.
-        if (!GT) same = match_any(ins ? h : 0xFFFF0000u | lane);
-        uint32_t pre_bit = 0;
-        if (taken && lane + L - 1 < 32) pre_bit = 1u << (lane + L - 1);
-        const uint32_t PRE = reduce_or(pre_bit);
-        const bool victim = ins && !((PRE >> lane) & 1u) && (same & C & ((1u << lane) - 1u)) != 0;
-        const uint32_t vm = ballot(victim);
-        if (vm) cut = ffs(vm) - 1;
-        // restore, then commit only the accepted prefix with "highest lane of a slot wins"
+        // Two inserted positions share a slot. A probed position with an earlier inserted position of the same
+        // slot should have seen that one as its candidate ("victim"): everything before the first victim is still
+        // exactly what the serial encoder does, so keep that prefix and restart the step at the victim. Copy-end
+        // pre-inserts (e-1) are write-only, never victims. Pairs within a half are found with match.any; a half-1
+        // position whose slot holds a half-0 one is found by re-reading the table with only half 0 committed.
+        const uint32_t same0 = match_any(ins0 ? h0 : 0xFFFF0000u | lane);
+        const uint32_t same1 = match_any(ins1 ? h1 : 0xFFFF0000u | lane);
+        uint64_t pre_bit = 0;
+        if (taken0 && lane + L0 - 1 < 64) pre_bit |= 1ull << (lane + L0 - 1);
+        if (taken1 && lane + L1 - 1 < 32) pre_bit |= 1ull << (32 + lane + L1 - 1);
+        const uint32_t PRE0 = reduce_or((uint32_t)pre_bit), PRE1 = reduce_or((uint32_t)(pre_bit >> 32));
+        // restore (same-slot lanes restore the same value), then commit the accepted prefix of half 0 with "highest
+        // position of a slot wins"
         syncwarp();
-        if (ins) table[h] = (uint16_t)c;
+        if (ins0) table[h0] = (uint16_t)c0;
+        if (ins1) table[h1] = (uint16_t)c1;
         syncwarp();
-        const uint32_t keep = C & (cut >= 32 ? 0xFFFFFFFFu : ((1u << cut) - 1u));
-        if (((keep >> lane) & 1u) && (same & keep & ~((2u << lane) - 1u)) == 0) table[h] = (uint16_t)p;
+        const uint32_t v0 = ballot(ins0 && !((PRE0 >> lane) & 1u) && (same0 & C0 & below) != 0);
+        uint32_t cut = v0 ? ffs(v0) - 1 : 64;                    // step accepted up to (not including) this position
+        const uint32_t keep0 = C0 & (cut >= 32 ? 0xFFFFFFFFu : ((1u << cut) - 1u));
+        if (((keep0 >> lane) & 1u) && (same0 & keep0 & above) == 0) table[h0] = (uint16_t)p0;
         syncwarp();
-        if (cut < 32) {
-            CS &= (1u << cut) - 1u;
-            const uint32_t ncut = popc(CS);
+        if (cut == 64) {
+            // half 0 is committed whole: a half-1 slot that no longer holds its candidate holds a half-0 position
+            const bool cross = ins1 && table[h1] != (uint16_t)c1;
+            const uint32_t v1 = ballot(ins1 && !((PRE1 >> lane) & 1u) && (cross || (same1 & C1 & below) != 0));
+            if (v1) cut = 32 + ffs(v1) - 1;
+            const uint32_t keep1 = C1 & (cut >= 64 ? 0xFFFFFFFFu : ((1u << (cut - 32)) - 1u));
+            syncwarp();
+            if (((keep1 >> lane) & 1u) && (same1 & keep1 & above) == 0) table[h1] = (uint16_t)p1;
+            syncwarp();
+        }
+        if (cut < 64) {
+            if (cut < 32) { CS0 &= (1u << cut) - 1u; CS1 = 0; }
+            else CS1 &= (1u << (cut - 32)) - 1u;
+            const bool t0 = (CS0 >> lane) & 1u, t1 = (CS1 >> lane) & 1u;
+            const uint32_t n0 = popc(CS0), ncut = n0 + popc(CS1);
+            k1_push_copies(ring, head, ncut, t0, popc(CS0 & below), k1_event(p0, L0, p0 - c0),
+                           t1, n0 + popc(CS1 & below), k1_event(p1, L1, p1 - c1));
             if (ncut) {
-                k1_wait_space(ring, head, ncut);
-                if ((CS >> lane) & 1u) ring.ev[(head.head + popc(CS & ((1u << lane) - 1u))) & (ring.size - 1)] = k1_event(p, L, p - c);
-                head.head += ncut;
-                if (head.head - head.published >= K1_PUBLISH) k1_publish(ring, head);
-                const unsigned lastc = 31 - clz(CS);
-                const uint32_t e2 = lastc + shfl(L, lastc);        // <= cut: the victim is not inside a copy
+                const uint32_t e2 = reduce_max(t1 ? 32 + lane + L1 : t0 ? lane + L0 : 0u);   // <= cut: the victim is not inside a copy
                 if (e2 == cut) { st.s = w + cut; st.rematch = true; }
                 else { st.s = w + cut; st.rematch = false; st.skip = 32 + (cut - e2 - 1); }
             } else {
@@ -433,53 +491,52 @@ SB_DEVICE bool k1_finish(const uint8_t* win, uint32_t n, uint16_t* table, unsign
     K1_TICK(5);                                                  // [5] commit + verify (+ clash handling)
     // ---- exit state and copy-end insert
     // (warp-uniform values, written as selects: only the copy-end insert below is a branch)
-    const uint32_t ncopy = popc(CS);
-    // hash of the word at e - 1 for a copy ending at e in 33..64 (the copy-end insert below), fetched by every lane for
+    const uint32_t n0 = popc(CS0), ncopy = n0 + popc(CS1);
+    // the end of the lane's last copy: its half-1 one when taken (a taken half-0 copy that reaches 32 + lane covers it)
+    const uint32_t e_mine = taken1 ? 32 + lane + L1 : taken0 ? lane + L0 : 0u;
+    // hash of the word at e - 1 for a copy ending at e in 65..96 (the copy-end insert below), fetched by every lane for
     // its own copy end while the reduction that finds the last copy runs, instead of by index after it
-    const unsigned nsh = (unsigned)((uintptr_t)(win + nxt->w + lane) & 3u) * 8;
-    const uint32_t hend = shfl(K1_HASH(funnel_r(nxt->a0, nxt->a1, nsh)), (lane + L - 33) & 31u);
-    const uint32_t e_last = reduce_max(taken ? lane + L : 0u);    // end of the window's last copy, 0 without one
-    const bool over = e_last >= 32;                               // that copy ends at or beyond the window's end
-    // else the window ends in a scan: probes since the last copy end, since the rematch miss at i0, or the running scan's
-    const uint32_t scan_skip = CS ? 32 + (31 - e_last) : st.rematch ? 32 + (31 - i0) : st.skip + (32 - i0);
-    st.s = w + (over ? e_last : 32);
+    const unsigned nsh = (unsigned)((uintptr_t)(win + nxt[0].w + lane) & 3u) * 8;
+    const uint32_t hend = shfl(K1_HASH(funnel_r(nxt[0].a0, nxt[0].a1, nsh)), (e_mine - 65) & 31u);
+    const uint32_t e_last = reduce_max(e_mine);                  // end of the step's last copy, 0 without one
+    const bool over = e_last >= 64;                              // that copy ends at or beyond the step's end
+    // else the step ends in a scan: probes since the last copy end, since the rematch miss at i0, or the running scan's
+    const uint32_t scan_skip = (CS0 | CS1) ? 32 + (63 - e_last) : st.rematch ? 32 + (63 - i0) : st.skip + (64 - i0);
+    st.s = w + (over ? e_last : 64);
     st.skip = over ? st.skip : scan_skip;
     st.rematch = over;
-    if (e_last >= 33) {                                       // e-1 lies beyond this window
-        if (nxt->w == w + 32 && e_last <= 64) {
-            // ... but inside the next one, whose sequential words are already prefetched: take
+    if (e_last >= 65) {                                          // e-1 lies beyond this step
+        if (nxt[0].w == w + 64 && e_last <= 96) {
+            // ... but inside the next step's first half, whose sequential words are already prefetched: take
             // its hash from the lane that holds it instead of paying a global load (:293-295)
             if (st.s < s_limit) {
                 syncwarp();
-                if (taken && lane + L == e_last) table[hend] = (uint16_t)(st.s - 1);   // the last copy's lane
+                if (e_mine == e_last) table[hend] = (uint16_t)(st.s - 1);   // the last copy's lane
                 syncwarp();
             }
         } else {
             k1_preinsert(win, table, shift, s_limit, st.s);
         }
     }
-    const uint32_t slot = popc(CS & ((1u << lane) - 1u));     // this lane's event among the window's copies
+    const uint32_t slot0 = popc(CS0 & below), slot1 = n0 + popc(CS1 & below);   // this lane's events among the step's
     K1_TICK(7);                                                  // [7] exit state / copy-end insert
-    // ---- the next window's probe. Every table store of this window is done, so when the next window is w + 32
-    // on the fast path its probe reads exactly the table it would read later: issue it now so that its candidate
-    // loads overlap the ring stores and the next window's prefetch (k1_parse keeps such windows in its inner loop)
-    hoisted = nxt->w == w + 32 && (st.s & ~31u) == w + 32 && k1_fast(w + 32, st, s_limit);
-    if (hoisted) nextp = k1_probe_issue(win, table, shift, *nxt);
-    // ---- publish the copies
-    if (ncopy) {
-        k1_wait_space(ring, head, ncopy);
-        if (taken) ring.ev[(head.head + slot) & (ring.size - 1)] = k1_event(p, L, p - c);
-        head.head += ncopy;
-        if (head.head - head.published >= K1_PUBLISH) k1_publish(ring, head);
+    // ---- the next step's probe. Every table store of this step is done, so when the next step is w + 64 on the
+    // fast path its probe reads exactly the table it would read later: issue it now so that its candidate loads
+    // overlap the ring stores and the next step's prefetch (k1_parse keeps such steps in its inner loop)
+    hoisted = nxt[0].w == w + 64 && (st.s & ~31u) == w + 64 && k1_fast(w + 64, st, s_limit);
+    if (hoisted) {
+        nextp[0] = k1_probe_issue(win, table, shift, nxt[0]);
+        nextp[1] = k1_probe_issue(win, table, shift, nxt[1]);
     }
+    // ---- publish the copies
+    k1_push_copies(ring, head, ncopy, taken0, slot0, k1_event(p0, L0, p0 - c0), taken1, slot1, k1_event(p1, L1, p1 - c1));
     K1_TICK(6);                                                  // [6] probe issue + event ring
     return true;
 }
 
-// Parser warp: block visible through `win` (global memory), n >= 17. One 32-position window per step;
-// the sequential words of the next window are requested before the current one is probed.
+// Parser warp: block visible through `win` (global memory), n >= 17. One 64-position step at a time;
+// the sequential words of the next step are requested before the current one is probed.
 //   ctrl[6..7] = ring producer counters (head, published), carried from unit to unit
-template <bool GT>
 SB_DEVICE void k1_parse(const uint8_t* win, uint32_t n, uint16_t* table, const K1Ring& ring, uint32_t* ctrl) {
     const unsigned lane = lane_id();
     unsigned shift = 24;
@@ -488,59 +545,67 @@ SB_DEVICE void k1_parse(const uint8_t* win, uint32_t n, uint16_t* table, const K
     const uint32_t s_limit = n - 15;
     K1Prod prod;
     prod.head = ld_volatile(&ctrl[6]); prod.published = ld_volatile(&ctrl[7]); prod.tail_seen = 0;
-    K1Seq seq;
-    seq.a0 = seq.a1 = seq.a2 = seq.a3 = seq.a4 = 0; seq.w = 0xFFFFFFFFu;
+    K1Seq seq[2];
+    seq[0].a0 = seq[0].a1 = seq[0].a2 = seq[0].a3 = seq[0].a4 = 0; seq[0].w = 0xFFFFFFFFu;
+    seq[1] = seq[0];
     K1_PROF_DECL
     K1State st;
     st.s = 1; st.skip = 32; st.rematch = false;
     for (;;) {
         uint32_t w = st.s & ~31u;
         bool finished;
-        // fast-path test first: when it holds (w + 36 < s_limit, stride 1) neither end-of-block test can
+        // fast-path test first: when it holds (w + 68 < s_limit, stride 1) neither end-of-block test can
         const bool fast = k1_fast(w, st, s_limit);
         if (!fast && (st.rematch ? st.s >= s_limit : st.s + (st.skip >> 5) > s_limit)) finished = true;
         else {
             bool ok = false;
             if (fast) {
-                K1Seq nxt = seq;
-                if (w + 100 < n) nxt = k1_fetch_seq(win, w + 32, n);   // issue next window's loads now
+                // the next step's words, when a step at w + 64 can run on the fast path: issue their loads now
+                K1Seq nxt[2] = {seq[0], seq[1]};
+                if (w + 64 + 68 < s_limit) { nxt[0] = k1_fetch_seq(win, w + 64, n); nxt[1] = k1_fetch_seq(win, w + 96, n); }
                 K1_TICK(0);                                          // [0] loop top / state checks / prefetch issue
-                K1Seq cur = seq.w == w ? seq : k1_fetch_seq(win, w, n);
-                K1Probe pb = k1_probe_issue(win, table, shift, cur);
+                K1Seq cur[2];
+                cur[0] = seq[0].w == w ? seq[0] : k1_fetch_seq(win, w, n);
+                cur[1] = seq[1].w == w + 32 ? seq[1] : k1_fetch_seq(win, w + 32, n);
+                K1Probe pb[2];
+                pb[0] = k1_probe_issue(win, table, shift, cur[0]);
+                pb[1] = k1_probe_issue(win, table, shift, cur[1]);
                 K1_COUNT(1);
-                // While a window issues its successor's probe (`hoisted`), the successor runs in this inner loop
+                // While a step issues its successor's probe (`hoisted`), the successor runs in this inner loop
                 // and not from the loop top: there the compiler joins all paths of the parse and waits for every
                 // load in flight, which would put the candidate loads back on the critical path. For the same
                 // reason the successor's own prefetch is issued only after its candidates are compared.
                 K1_TICK(11);                                         // [11] probe issue (loop top)
 #ifdef SB_EMU
-                if (table[pb.h] != (uint16_t)pb.c) K1_COUNT(2);
+                if (any(table[pb[0].h] != (uint16_t)pb[0].c || table[pb[1].h] != (uint16_t)pb[1].c)) K1_COUNT(2);
 #endif
                 K1Pre pre = k1_probe_complete(win, cur, pb);
                 K1_TICK(1);                                          // [1] candidate wait, compare, doubling
                 for (;;) {
-                    seq = nxt;
+                    seq[0] = nxt[0]; seq[1] = nxt[1];
                     bool hoisted;
-                    ok = k1_finish<GT>(win, n, table, shift, s_limit, st, ring, prod, pre, &seq, pb, hoisted K1_PROF_PASS);
+                    ok = k1_finish(win, n, table, shift, s_limit, st, ring, prod, pre, seq, pb, hoisted K1_PROF_PASS);
                     if (!hoisted) break;
-                    w += 32;                                         // == st.s & ~31u, on the fast path
-                    cur = seq;
+                    w += 64;                                         // == st.s & ~31u, on the fast path
+                    cur[0] = seq[0]; cur[1] = seq[1];
                     K1_TICK(0);
                     K1_COUNT(0);
 #ifdef SB_EMU
-                    if (table[pb.h] != (uint16_t)pb.c) K1_COUNT(2);
+                    if (any(table[pb[0].h] != (uint16_t)pb[0].c || table[pb[1].h] != (uint16_t)pb[1].c)) K1_COUNT(2);
 #endif
                     pre = k1_probe_complete(win, cur, pb);
                     K1_TICK(1);
-                    // unconditional (the current window when w + 32 is too close to the end): a conditional load
+                    // unconditional (this step's own words when w + 64 cannot be a fast step): a conditional load
                     // would become register moves that wait for it
-                    nxt = k1_fetch_seq(win, w + 100 < n ? w + 32 : w, n);
-                    // the words four windows ahead come from HBM: have L2 fetch them now, so that the load above
-                    // finds them in L2 when its turn comes (a prefetch has no register to wait for)
-                    prefetch_l2(win + (w + 128 + lane < n ? w + 128 + lane : n - 1));
+                    const bool ahead = w + 64 + 68 < s_limit;
+                    nxt[0] = k1_fetch_seq(win, ahead ? w + 64 : w, n);
+                    nxt[1] = k1_fetch_seq(win, ahead ? w + 96 : w + 32, n);
+                    // the words that the next step fetches come from HBM: have L2 fetch them now, so that the
+                    // load finds them in L2 when its turn comes (a prefetch has no register to wait for)
+                    prefetch_l2(win + (w + 160 + 2 * lane < n ? w + 160 + 2 * lane : n - 1));
                 }
             }
-            if (!ok) { K1_TICK(8); finished = k1_serial(win, n, table, shift, s_limit, st, w + 32, ring, prod); K1_TICK(9); }   // [9] serial path
+            if (!ok) { K1_TICK(8); finished = k1_serial(win, n, table, shift, s_limit, st, w + 64, ring, prod); K1_TICK(9); }   // [9] serial path
             else finished = false;
         }
         if (finished) {
@@ -652,7 +717,7 @@ SB_DEVICE uint32_t k1_emit_block(const uint8_t* win, uint8_t* out, uint32_t d, c
 // status array, TooBig / BufferTooSmall with the reference's payloads (src/compress.rs:104-117).
 // The role is a template argument so that the parser's code does not keep the emitter's state (ring tail, output
 // pointer) live across the parse: with one shared body the 7 + 5 and 7 + 7 kernels spill under their register caps.
-template <bool GT, bool parser>
+template <bool parser>
 SB_DEVICE void k1_chain(const BatchDesc& b, uint32_t flags, uint16_t* table, const K1Ring& ring, uint32_t* ctrl,
                         uint32_t* work, unsigned bar, uint32_t* crcs, const uint32_t* crc_tab) {
     const unsigned lane = lane_id();
@@ -698,7 +763,7 @@ SB_DEVICE void k1_chain(const BatchDesc& b, uint32_t flags, uint16_t* table, con
         }
         bar_sync(bar, 64);
         if (parser) {
-            if (n >= 17) k1_parse<GT>(in, n, table, ring, ctrl);           // (:140-150)
+            if (n >= 17) k1_parse(in, n, table, ring, ctrl);           // (:140-150)
             else {                                                         // tiny block: one literal (:140-146)
                 K1Prod prod;
                 prod.head = ctrl[6]; prod.published = ctrl[7]; prod.tail_seen = 0;
@@ -741,12 +806,12 @@ SB_DEVICE void k1_compress_body_multi(const BatchDesc& b, uint32_t flags, uint64
     ring.ctrl = ctrl;
     if (NG == 0 || c < NC) {
         uint16_t* table = (uint16_t*)(sm + (size_t)c * K1_TABLE_BYTES);
-        if (parser) k1_chain<false, true>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
-        else k1_chain<false, false>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
+        if (parser) k1_chain<true>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
+        else k1_chain<false>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
     } else {
         uint16_t* table = gtables + ((size_t)block_idx() * NG + (c - NC)) * (K1_TABLE_BYTES / 2);
-        if (parser) k1_chain<true, true>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
-        else k1_chain<true, false>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
+        if (parser) k1_chain<true>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
+        else k1_chain<false>(b, flags, table, ring, ctrl, work, 1 + c, crcs, crc_tab);
     }
 }
 

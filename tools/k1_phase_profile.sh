@@ -40,12 +40,13 @@ names = ["loop top/prefetch", "probe: candidate wait, compare", "pointer doublin
          "block end", "probe issue at the loop top"]
 tot = sum(out[i] for i in range(12))
 windows = n * (BLOCK // 32)
-print("lib %s: kernel %.2f ms, %.2f GB/s; parser cycles per 32-byte window: %.0f"
-      % (os.path.basename(os.environ["SNAPB200_LIB"]), e0.elapsed_time(e1), n * BLOCK / e0.elapsed_time(e1) / 1e6, tot / windows))
-for i in range(12):
-    print("  [%2d] %-34s %6.1f%%  %7.0f cyc/window" % (i, names[i], 100.0 * out[i] / tot, out[i] / windows))
-print("parser warps per scheduler (%%warpid & 3 = 0..3): %s" % [out[12 + s] for s in range(4)])
 fw = out[16] + out[17]
-print("fast-path windows: %d; probe issued by the previous window (hoisted): %d (%.1f%%), at the loop top: %d"
-      % (fw, out[16], 100.0 * out[16] / max(fw, 1), out[17]))
+print("lib %s: kernel %.2f ms, %.2f GB/s; parser cycles per 32 input bytes: %.0f, per fast-path step: %.0f"
+      % (os.path.basename(os.environ["SNAPB200_LIB"]), e0.elapsed_time(e1), n * BLOCK / e0.elapsed_time(e1) / 1e6,
+         tot / windows, tot / max(fw, 1)))
+for i in range(12):
+    print("  [%2d] %-34s %6.1f%%  %7.0f cyc/32 B" % (i, names[i], 100.0 * out[i] / tot, out[i] / windows))
+print("parser warps per scheduler (%%warpid & 3 = 0..3): %s" % [out[12 + s] for s in range(4)])
+print("fast-path steps: %d (%.0f per block); probe issued by the previous step (hoisted): %d (%.1f%%), at the loop top: %d"
+      % (fw, fw / n, out[16], 100.0 * out[16] / max(fw, 1), out[17]))
 PY

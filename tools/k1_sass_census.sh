@@ -5,10 +5,10 @@
 # count and the counts of the instructions that cost more than an issue slot (SHFL, VOTE, REDUX, MATCH, FLO, shared
 # and global loads/stores, BSSY = divergent regions to reconverge from), plus every K1 kernel's registers and spills
 # from -Xptxas -v. In k1_m7_kernel<0> the first large loop is the emitter's, the largest the chain's loop over units;
-# nested in that one are the parse loop of k1_parse, in it the loop of windows whose probe the previous window issued
+# nested in that one are the parse loop of k1_parse, in it the loop of steps whose probe the previous step issued
 # (k1_probe_complete + k1_finish), and beside that the serial path.
-# A static count is a rehearsal metric: it is not a time and says nothing about which instructions a window executes.
-# WAITS=1 adds the scoreboard table of one loop (HEAD=0x..., default the largest loop at depth 2: the loop of windows
+# A static count is a rehearsal metric: it is not a time and says nothing about which instructions a step executes.
+# WAITS=1 adds the scoreboard table of one loop (HEAD=0x..., default the largest loop at depth 2: the loop of steps
 # whose probe was issued early). Every instruction's control bits are decoded from the high word of its 128-bit
 # encoding (bits 41..44 stall cycles, 45 yield, 46..48 write scoreboard, 49..51 read scoreboard, 7 = none, 52..57 wait
 # mask); the per-instruction listing goes to $OUT/census.ctrl. For every instruction of the loop that sets a scoreboard
