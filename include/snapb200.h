@@ -75,6 +75,12 @@ int sb_decompress_len(const uint8_t* in, size_t n, size_t* out_len, sb_error* er
  * variant and payload of the reference on corrupt input. */
 int sb_decompress(const uint8_t* in, size_t n, uint8_t* out, size_t cap, size_t* out_n, sb_error* err);
 
+/* Validation of one raw stream without its decoded bytes: returns 0 with *out_len = the decoded length exactly when
+ * sb_decompress(in, n, buf, decompressed length, ...) succeeds, and otherwise that call's error (variant and payload).
+ * Empty input is Empty and n above 2^32 - 1 SB_E_INVALID, as in sb_decompress. The stream runs through
+ * sb_validate_batch_device_ws as a batch of one; no decoded byte is written anywhere. */
+int sb_validate(const uint8_t* in, size_t n, size_t* out_len, sb_error* err);
+
 /* Stream-ordered raw decode of one stream d_in[0..n) in device memory into d_out[0..cap), caller scratch of
  * sb_decompress_scratch_bytes(n) bytes (sized from the compressed length alone), no allocation, no host
  * synchronisation. The stream's 64 KB blocks are located on the device and decoded in parallel, one warp per block;
@@ -156,6 +162,16 @@ int sb_decompress_batch_device(const sb_batch* batch, void* stream, sb_error* er
 uint64_t sb_decompress_batch_scratch_bytes(uint32_t count, uint64_t in_bytes);
 int sb_decompress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t* d_unit_blocks,
                                   void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
+/* Validation of a batch of raw streams without their decoded bytes: statuses[i], out_lens[i] and d_unit_blocks[i] are
+ * what sb_decompress_batch_device_ws gives unit i with out_caps[i] = 2^32 - 1 (Ok with the decoded length, or the
+ * reference's error with out_lens 0), and the split and block checks are the same, but no decoded byte is written:
+ * K2's element loop makes every error decision from element positions alone. out_ptrs, out_base, out_stride, out_caps
+ * and out_cap_uniform are ignored and may be null or zero; statuses and out_lens are required. The scratch is
+ * sb_decompress_batch_scratch_bytes(count, in_bytes) bytes and in_bytes means what it means there. Stream ordered, no
+ * allocation, no host synchronisation. Null pointers, count >= 2^31 and scratch that is too small are SB_E_INVALID
+ * with nothing launched; count == 0 does nothing. */
+int sb_validate_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t* d_unit_blocks,
+                                void* scratch, uint64_t scratch_bytes, void* stream, sb_error* err);
 /* Raw compress of units of ANY length: unit i becomes exactly what Encoder::compress(input_i, &mut output_i[..cap_i])
  * produces (src/compress.rs:99-154), cap_i = out_caps[i] or the uniform cap; the same addressing as the other batch
  * calls, and a uniform length over 65536 is legal. Every unit is cut into its 64 KB blocks and the blocks of all units
@@ -230,6 +246,21 @@ int sb_frame_decode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, ui
                                     const uint64_t* d_chunk_offs, const uint64_t* d_index_at, uint32_t max_chunks,
                                     uint32_t* d_unit_chunks, void* scratch, uint64_t scratch_bytes,
                                     void* stream, sb_error* err);
+/* Validation of a batch of frame streams without their decoded bytes: statuses[i], out_lens[i] and d_unit_chunks[i]
+ * are what sb_frame_decode_batch_device_ws (same flags, index, in_bytes and max_chunks) gives unit i with every cap
+ * 2^32 - 1: Ok with the decoded length, the reader's first error with the bytes produced before it, SB_E_INVALID{a=
+ * max_chunks, b=1} when the chunk table is too small, and BufferTooSmall{given=2^32 - 1, min=decoded length} for a
+ * unit that decodes to more. Compressed chunks are decoded into a pool of min(max_chunks, 4,096) staging slots of 64 KiB
+ * in the scratch and checksummed there; stored chunks are checksummed in place. out_ptrs, out_base, out_stride, out_caps
+ * and out_cap_uniform are ignored and may be null or zero; statuses and out_lens are required. The scratch,
+ * sb_frame_validate_batch_scratch_bytes(count, in_bytes, max_chunks) bytes, is the decode call's plus the slot pool
+ * and a 256-byte work counter (at most 256 MiB + 256 bytes more) and depends on nothing else. Stream ordered, no
+ * allocation, no host synchronisation; the argument checks are the decode call's. */
+uint64_t sb_frame_validate_batch_scratch_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks);
+int sb_frame_validate_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t flags,
+                                      const uint64_t* d_chunk_offs, const uint64_t* d_index_at, uint32_t max_chunks,
+                                      uint32_t* d_unit_chunks, void* scratch, uint64_t scratch_bytes,
+                                      void* stream, sb_error* err);
 /* Masked CRC-32C of each unit (frame chunks): out_lens[i] receives the CRC. */
 int sb_crc32c_masked_batch_device(const sb_batch* batch, void* stream, sb_error* err);
 
@@ -591,11 +622,14 @@ int sb_bind_host_thread_to_device_numa(int device);
  * (snappy-cpp/src/lib.rs:66-88, snappy-c.h): linking the reference's test/ and
  * bench/ crates with `--features cpp` against this library runs their
  * cross-implementation tests on the GPU codec. 0 = SNAPPY_OK, 1 = INVALID_INPUT,
- * 2 = BUFFER_TOO_SMALL. */
+ * 2 = BUFFER_TOO_SMALL. snappy_validate_compressed_buffer, the fifth function of
+ * snappy-c.h, is 0 exactly when sb_validate succeeds (so when snappy_uncompress
+ * succeeds given a buffer of the decoded length), else 1. */
 int snappy_compress(const char* input, size_t input_length, char* compressed, size_t* compressed_length);
 int snappy_uncompress(const char* compressed, size_t compressed_length, char* uncompressed, size_t* uncompressed_length);
 size_t snappy_max_compressed_length(size_t source_length);
 int snappy_uncompressed_length(const char* compressed, size_t compressed_length, size_t* result);
+int snappy_validate_compressed_buffer(const char* compressed, size_t compressed_length);
 
 /* ---- misc ---------------------------------------------------------------- */
 /* Number of kernel launches issued by this library since load (bench.py's

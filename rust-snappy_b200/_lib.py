@@ -32,14 +32,15 @@ class SbBatch(C.Structure):
 
 # every symbol include/snapb200.h declares
 SYMBOLS = [
-    "sb_max_compress_len", "sb_compress", "sb_decompress_len", "sb_decompress", "sb_decompress_scratch_bytes",
+    "sb_max_compress_len", "sb_compress", "sb_decompress_len", "sb_decompress", "sb_validate", "sb_decompress_scratch_bytes",
     "sb_decompress_device_ws", "sb_crc32c_masked",
     "sb_compress_batch_host", "sb_decompress_batch_host", "sb_compress_batch_host_packed",
     "sb_compress_batch_device", "sb_decompress_batch_device", "sb_decompress_batch_scratch_bytes",
-    "sb_decompress_batch_device_ws", "sb_compress_batch_scratch_bytes", "sb_compress_batch_device_ws",
+    "sb_decompress_batch_device_ws", "sb_validate_batch_device_ws", "sb_compress_batch_scratch_bytes", "sb_compress_batch_device_ws",
     "sb_crc32c_masked_batch_device",
     "sb_frame_encode_batch_scratch_bytes", "sb_frame_encode_batch_device_ws",
     "sb_frame_decode_batch_scratch_bytes", "sb_frame_decode_batch_device_ws",
+    "sb_frame_validate_batch_scratch_bytes", "sb_frame_validate_batch_device_ws",
     "sb_frame_decode_ranges_scratch_bytes", "sb_frame_decode_ranges_device_ws",
     "sb_frame_table_bytes", "sb_frame_table_build_scratch_bytes", "sb_frame_table_build_device_ws",
     "sb_frame_table_ranges_scratch_bytes", "sb_frame_table_decode_ranges_device_ws",
@@ -59,6 +60,7 @@ SYMBOLS = [
     "sb_bind_host_thread_to_device_numa",
     "sb_launch_count", "sb_generate_blocks_device", "sb_version",
     "snappy_compress", "snappy_uncompress", "snappy_max_compressed_length", "snappy_uncompressed_length",
+    "snappy_validate_compressed_buffer",
 ]
 
 _lib = None
@@ -84,6 +86,7 @@ def lib():
     L.sb_compress.argtypes = [vp, sz, vp, sz, szp, ep]
     L.sb_decompress_len.argtypes = [vp, sz, szp, ep]
     L.sb_decompress.argtypes = [vp, sz, vp, sz, szp, ep]
+    L.sb_validate.argtypes = [vp, sz, szp, ep]
     L.sb_decompress_scratch_bytes.restype = C.c_uint64
     L.sb_decompress_scratch_bytes.argtypes = [C.c_uint64]
     L.sb_decompress_device_ws.argtypes = [vp, C.c_uint64, vp, C.c_uint64, vp, vp, C.c_uint64, vp, ep]
@@ -95,6 +98,7 @@ def lib():
     L.sb_decompress_batch_scratch_bytes.restype = C.c_uint64
     L.sb_decompress_batch_scratch_bytes.argtypes = [C.c_uint32, C.c_uint64]
     L.sb_decompress_batch_device_ws.argtypes = [C.POINTER(SbBatch), C.c_uint64, vp, vp, C.c_uint64, vp, ep]
+    L.sb_validate_batch_device_ws.argtypes = [C.POINTER(SbBatch), C.c_uint64, vp, vp, C.c_uint64, vp, ep]
     L.sb_compress_batch_scratch_bytes.restype = C.c_uint64
     L.sb_compress_batch_scratch_bytes.argtypes = [C.c_uint32, C.c_uint64]
     L.sb_compress_batch_device_ws.argtypes = [C.POINTER(SbBatch), C.c_uint64, vp, C.c_uint64, vp, ep]
@@ -105,6 +109,9 @@ def lib():
     L.sb_frame_decode_batch_scratch_bytes.argtypes = [C.c_uint32, C.c_uint64, C.c_uint32]
     L.sb_frame_decode_batch_device_ws.argtypes = [C.POINTER(SbBatch), C.c_uint64, C.c_uint32, vp, vp, C.c_uint32, vp, vp,
                                                   C.c_uint64, vp, ep]
+    L.sb_frame_validate_batch_scratch_bytes.restype = C.c_uint64
+    L.sb_frame_validate_batch_scratch_bytes.argtypes = [C.c_uint32, C.c_uint64, C.c_uint32]
+    L.sb_frame_validate_batch_device_ws.argtypes = L.sb_frame_decode_batch_device_ws.argtypes
     L.sb_frame_decode_ranges_scratch_bytes.restype = C.c_uint64
     L.sb_frame_decode_ranges_scratch_bytes.argtypes = [C.c_uint32, C.c_uint32]
     L.sb_frame_decode_ranges_device_ws.argtypes = [vp, C.c_uint64, vp, C.c_uint32, C.c_uint32, vp, vp, vp, vp, vp, C.c_uint32,
@@ -183,5 +190,6 @@ def lib():
     L.snappy_compress.argtypes = [vp, sz, vp, szp]
     L.snappy_uncompress.argtypes = [vp, sz, vp, szp]
     L.snappy_uncompressed_length.argtypes = [vp, sz, szp]
+    L.snappy_validate_compressed_buffer.argtypes = [vp, sz]
     _lib = L
     return L

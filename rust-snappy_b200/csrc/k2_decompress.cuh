@@ -39,8 +39,10 @@ SB_DEVICE uint32_t k2_read_header(const uint8_t* in, uint32_t n, uint64_t* value
 // Decode one raw stream with the calling warp. Returns the status code. kHeader = false: `in` is the element sequence
 // of one block alone (no varint header) that must produce exactly `cap` bytes -- K8 (k8_raw_split.cuh) hands every
 // block of a split stream to its own warp this way, and the reference's checks are then made against the block's
-// bounds, which are stricter than the stream's.
-template <bool kHeader = true>
+// bounds, which are stricter than the stream's. kStore = false validates without output: the literal scatter, the copies
+// and the spill's copy are compiled out, so `dst` is never touched and `elems` may be null; the window advance, every
+// check, the status and *out_len are the same as with kStore = true (no error decision reads a decoded byte).
+template <bool kHeader = true, bool kStore = true>
 SB_DEVICE uint32_t k2_decode_stream(const uint8_t* in, uint32_t n, uint8_t* dst, uint64_t cap,
                                     sb_error* st, uint32_t* out_len, uint32_t* elems) {
     const unsigned lane = lane_id();
@@ -140,87 +142,89 @@ SB_DEVICE uint32_t k2_decode_stream(const uint8_t* in, uint32_t n, uint8_t* dst,
             }
         }
 
-        // ---- literal payload bytes that sit inside the window: lane -> output byte
-        {
-            const unsigned own = 31 - clz(M & (0xFFFFFFFFu >> (31 - lane)));  // nearest start <= lane
-            const uint32_t pk = shfl((opos << 8) | (hdr << 4) | (kind << 1) | (spill ? 1u : 0u), own);
-            const unsigned ohdr = (pk >> 4) & 0xFu;
-            if (valid && (pk & 7u) == 0 && lane >= own + ohdr)
-                dst[d + (pk >> 8) + (lane - own - ohdr)] = (uint8_t)tag;
-        }
-        syncwarp();
-
-        // ---- copies. A copy whose source lies entirely before this window's output
-        // (offset >= opos + len) depends on nothing written in this window. Those are flattened:
-        // their bytes form one compact index space, one lane per copied byte, so a window's
-        // ~30-60 copied bytes move in one or two warp-wide load/store pairs regardless of how many
-        // copies they belong to. The rest (recent/overlapping sources, lengths above 32) are
-        // replayed one by one in stream order afterwards.
-        {
-            uint8_t* const wout = dst + d;                       // window output base
-            const uint32_t cpk = opos | ((uint32_t)len << 12);   // len <= 64 for copies, opos <= 2048
-            const bool is_copy = is_start && kind != 0;
-            const bool indep = is_copy && (uint32_t)len <= 32 && off >= opos + (uint32_t)len;
-            const uint32_t im = ballot(indep);
-            if (im) {
-                // compact index of my first byte = prefix sum of independent copy lengths
-                const uint32_t ilen = indep ? (uint32_t)len : 0u;
-                uint32_t cincl = ilen;
-#pragma unroll
-                for (int k = 1; k < 32; k <<= 1) {
-                    const uint32_t t2 = shfl_up(cincl, k);
-                    if (lane >= (unsigned)k) cincl += t2;
-                }
-                const uint32_t cpos = cincl - ilen, ctot = shfl(cincl, 31);
-                // element table in shared memory, indexed by rank among the independent copies
-                if (indep) {
-                    const uint32_t rk = popc(im & ((1u << lane) - 1u));
-                    elems[rk * 2] = cpk | (cpos << 20);          // opos:12 | len:8 | cpos:12
-                    elems[rk * 2 + 1] = off;
-                }
-                syncwarp();
-                for (uint32_t base = 0; base < ctot; base += 64) {
-                    uint32_t dsto[2], srco[2];
-                    uint8_t v[2];
-                    bool on[2];
-#pragma unroll
-                    for (int q = 0; q < 2; q++) {
-                        const uint32_t lo = base + 32 * q;
-                        // starts inside [lo, lo+32) -> bit; owner rank of byte t = starts at or before t, minus one
-                        const uint32_t bit = (indep && cpos >= lo && cpos < lo + 32) ? 1u << (cpos - lo) : 0u;
-                        const uint32_t Bm = reduce_or(bit);
-                        const uint32_t before = popc(ballot(indep && cpos < lo));
-                        const uint32_t t = lo + lane;
-                        on[q] = t < ctot;
-                        const uint32_t rk = before + popc(Bm & (0xFFFFFFFFu >> (31 - lane))) - 1;
-                        const uint32_t e0 = on[q] ? elems[rk * 2] : 0u, e1 = on[q] ? elems[rk * 2 + 1] : 0u;
-                        dsto[q] = (e0 & 0xFFFu) + (t - (e0 >> 20));
-                        srco[q] = e1;
-                    }
-#pragma unroll
-                    for (int q = 0; q < 2; q++) v[q] = on[q] ? wout[(int64_t)dsto[q] - (int64_t)srco[q]] : (uint8_t)0;   // offsets up to 2^32-1 are legal (:433-474)
-#pragma unroll
-                    for (int q = 0; q < 2; q++) if (on[q]) wout[dsto[q]] = v[q];
-                }
+        if constexpr (kStore) {
+            // ---- literal payload bytes that sit inside the window: lane -> output byte
+            {
+                const unsigned own = 31 - clz(M & (0xFFFFFFFFu >> (31 - lane)));  // nearest start <= lane
+                const uint32_t pk = shfl((opos << 8) | (hdr << 4) | (kind << 1) | (spill ? 1u : 0u), own);
+                const unsigned ohdr = (pk >> 4) & 0xFu;
+                if (valid && (pk & 7u) == 0 && lane >= own + ohdr)
+                    dst[d + (pk >> 8) + (lane - own - ohdr)] = (uint8_t)tag;
             }
             syncwarp();
-            uint32_t cm = ballot(is_copy && !indep);
-            while (cm) {
-                const unsigned j = ffs(cm) - 1;
-                cm &= cm - 1;
-                const uint32_t pk1 = shfl(cpk, j), coff = shfl(off, j);
-                const uint32_t clen = pk1 >> 12;
-                uint8_t* out = wout + (pk1 & 0xFFFu);
-                if (coff >= clen || clen <= 32) {
-                    // lanes below the offset read final bytes; an overlapping short copy is the
-                    // periodic pattern of the last `coff` bytes (:306-317)
-                    if (lane < clen) out[lane] = out[(int64_t)(coff >= clen || lane < coff ? lane : lane % coff) - (int64_t)coff];
-                    if (clen > 32 && lane + 32 < clen) out[lane + 32] = out[(int64_t)lane + 32 - (int64_t)coff];
-                } else {
-                    const uint8_t* from = out - coff;
-                    for (uint32_t k = lane; k < clen; k += 32) out[k] = from[k % coff];
+
+            // ---- copies. A copy whose source lies entirely before this window's output
+            // (offset >= opos + len) depends on nothing written in this window. Those are flattened:
+            // their bytes form one compact index space, one lane per copied byte, so a window's
+            // ~30-60 copied bytes move in one or two warp-wide load/store pairs regardless of how many
+            // copies they belong to. The rest (recent/overlapping sources, lengths above 32) are
+            // replayed one by one in stream order afterwards.
+            {
+                uint8_t* const wout = dst + d;                       // window output base
+                const uint32_t cpk = opos | ((uint32_t)len << 12);   // len <= 64 for copies, opos <= 2048
+                const bool is_copy = is_start && kind != 0;
+                const bool indep = is_copy && (uint32_t)len <= 32 && off >= opos + (uint32_t)len;
+                const uint32_t im = ballot(indep);
+                if (im) {
+                    // compact index of my first byte = prefix sum of independent copy lengths
+                    const uint32_t ilen = indep ? (uint32_t)len : 0u;
+                    uint32_t cincl = ilen;
+#pragma unroll
+                    for (int k = 1; k < 32; k <<= 1) {
+                        const uint32_t t2 = shfl_up(cincl, k);
+                        if (lane >= (unsigned)k) cincl += t2;
+                    }
+                    const uint32_t cpos = cincl - ilen, ctot = shfl(cincl, 31);
+                    // element table in shared memory, indexed by rank among the independent copies
+                    if (indep) {
+                        const uint32_t rk = popc(im & ((1u << lane) - 1u));
+                        elems[rk * 2] = cpk | (cpos << 20);          // opos:12 | len:8 | cpos:12
+                        elems[rk * 2 + 1] = off;
+                    }
+                    syncwarp();
+                    for (uint32_t base = 0; base < ctot; base += 64) {
+                        uint32_t dsto[2], srco[2];
+                        uint8_t v[2];
+                        bool on[2];
+#pragma unroll
+                        for (int q = 0; q < 2; q++) {
+                            const uint32_t lo = base + 32 * q;
+                            // starts inside [lo, lo+32) -> bit; owner rank of byte t = starts at or before t, minus one
+                            const uint32_t bit = (indep && cpos >= lo && cpos < lo + 32) ? 1u << (cpos - lo) : 0u;
+                            const uint32_t Bm = reduce_or(bit);
+                            const uint32_t before = popc(ballot(indep && cpos < lo));
+                            const uint32_t t = lo + lane;
+                            on[q] = t < ctot;
+                            const uint32_t rk = before + popc(Bm & (0xFFFFFFFFu >> (31 - lane))) - 1;
+                            const uint32_t e0 = on[q] ? elems[rk * 2] : 0u, e1 = on[q] ? elems[rk * 2 + 1] : 0u;
+                            dsto[q] = (e0 & 0xFFFu) + (t - (e0 >> 20));
+                            srco[q] = e1;
+                        }
+#pragma unroll
+                        for (int q = 0; q < 2; q++) v[q] = on[q] ? wout[(int64_t)dsto[q] - (int64_t)srco[q]] : (uint8_t)0;   // offsets up to 2^32-1 are legal (:433-474)
+#pragma unroll
+                        for (int q = 0; q < 2; q++) if (on[q]) wout[dsto[q]] = v[q];
+                    }
                 }
                 syncwarp();
+                uint32_t cm = ballot(is_copy && !indep);
+                while (cm) {
+                    const unsigned j = ffs(cm) - 1;
+                    cm &= cm - 1;
+                    const uint32_t pk1 = shfl(cpk, j), coff = shfl(off, j);
+                    const uint32_t clen = pk1 >> 12;
+                    uint8_t* out = wout + (pk1 & 0xFFFu);
+                    if (coff >= clen || clen <= 32) {
+                        // lanes below the offset read final bytes; an overlapping short copy is the
+                        // periodic pattern of the last `coff` bytes (:306-317)
+                        if (lane < clen) out[lane] = out[(int64_t)(coff >= clen || lane < coff ? lane : lane % coff) - (int64_t)coff];
+                        if (clen > 32 && lane + 32 < clen) out[lane + 32] = out[(int64_t)lane + 32 - (int64_t)coff];
+                    } else {
+                        const uint8_t* from = out - coff;
+                        for (uint32_t k = lane; k < clen; k += 32) out[k] = from[k % coff];
+                    }
+                    syncwarp();
+                }
             }
         }
 
@@ -229,8 +233,10 @@ SB_DEVICE uint32_t k2_decode_stream(const uint8_t* in, uint32_t n, uint8_t* dst,
         if (lpk & 1u) {
             const uint32_t llen = shfl((uint32_t)len, last);   // validated above: fits in 32 bits
             const uint32_t lsrc = s + last + (lpk >> 1);
-            warp_copy(dst + d + win_out, src + lsrc, llen);
-            syncwarp();
+            if constexpr (kStore) {
+                warp_copy(dst + d + win_out, src + lsrc, llen);
+                syncwarp();
+            }
             s = lsrc + llen;
             d += win_out + llen;
         } else {

@@ -313,11 +313,14 @@ SB_DEVICE void k8_cuts_body(const RawPlan& p) {
                 [&] { return p.tiles[k / K4_TILE] + p.offs[k]; });
 }
 
-// block j of a split stream (dn: its decompressed length), decoded alone by the calling warp
+// block j of a split stream (dn: its decompressed length), decoded alone by the calling warp (kStore = false: validated,
+// nothing written)
+template <bool kStore = true>
 SB_DEVICE void k8_block(const RawPlan& p, uint64_t j, uint64_t dn, uint32_t* elems) {
     const uint32_t a = p.cut[j], b = p.cut[j + 1];
     const uint64_t want = dn - (j << 16) < 65536 ? dn - (j << 16) : 65536;
-    const uint32_t code = k2_decode_stream<false>(p.in + a, b - a, p.out + (j << 16), want, nullptr, nullptr, elems);
+    const uint32_t code = k2_decode_stream<false, kStore>(p.in + a, b - a, kStore ? p.out + (j << 16) : nullptr, want, nullptr,
+                                                          nullptr, elems);
     if (code != SB_OK && lane_id() == 0) p.ctl->decline = 1;
 }
 SB_DEVICE void k8_blocks_body(const RawPlan& p) {
@@ -361,6 +364,10 @@ SB_DEVICE void k8_fallback_body(const RawPlan& p) {
 //   k8b_blocks      warp per block of the global block list.
 //   k8b_finish      warp per unit, always: split units get Ok, dn and their block count; every other unit (never split,
 //                   or declined anywhere above) is decoded by k2_decode_stream exactly as k2_decompress_body does.
+// Validation (sb_validate_batch_device_ws) runs the same sequence with kStore = false in k8b_blocks and k8b_finish:
+// blocks and one-warp units are checked by K2's element loop without a decoded byte being written. The split steps
+// never write output; validation launches them on a copy of the batch without output pointers and with caps of
+// 2^32 - 1, so every header up to kMaxInput may split.
 // A unit is split only when it has more than one block, fits its output, and its header announces no more output than
 // its body can encode (64 bytes per 3-byte copy-2 is the densest element). That bounds the blocks by the compressed
 // bytes, so every slice is sized from the caller's bound `in_bytes` on Σ in_lens; when the lengths on the device sum
@@ -548,6 +555,7 @@ SB_DEVICE void k8b_cuts_body(const RawBatchPlan& q) {
                     [&] { return obase; });
     });
 }
+template <bool kStore = true>
 SB_DEVICE void k8b_blocks_body(const RawBatchPlan& q) {
     if (k8b_over(q)) return;
     uint32_t* elems = (uint32_t*)smem() + warp_id() * 64;
@@ -564,9 +572,10 @@ SB_DEVICE void k8b_blocks_body(const RawBatchPlan& q) {
             if (lane_id() == 0) p.ctl->decline = 1;
             continue;
         }
-        k8_block(p, j, p.ctl->dn, elems);
+        k8_block<kStore>(p, j, p.ctl->dn, elems);
     }
 }
+template <bool kStore = true>
 SB_DEVICE void k8b_finish_body(const RawBatchPlan& q) {
     const BatchDesc& b = q.b;
     const bool over = k8b_over(q);
@@ -588,8 +597,8 @@ SB_DEVICE void k8b_finish_body(const RawBatchPlan& q) {
             if (b.out_lens) b.out_lens[i] = 0;
             if (q.unit_blocks) q.unit_blocks[i] = 0;
         }
-        k2_decode_stream(unit_in(b, i), unit_in_len(b, i), unit_out(b, i), unit_out_cap(b, i),
-                         b.statuses ? &b.statuses[i] : nullptr, b.out_lens ? &b.out_lens[i] : nullptr, elems);
+        k2_decode_stream<true, kStore>(unit_in(b, i), unit_in_len(b, i), kStore ? unit_out(b, i) : nullptr, unit_out_cap(b, i),
+                                       b.statuses ? &b.statuses[i] : nullptr, b.out_lens ? &b.out_lens[i] : nullptr, elems);
     }
 }
 

@@ -30,6 +30,7 @@
 #include "k15_raw_table.cuh"
 #include "k16_encode_tables.cuh"
 #include "k17_table_gather.cuh"
+#include "k19_validate.cuh"
 
 namespace {
 
@@ -82,6 +83,8 @@ __global__ void __launch_bounds__(1024) k8b_scan_tiles_kernel(sbk::RawBatchPlan 
 __global__ void __launch_bounds__(128) k8b_cuts_kernel(sbk::RawBatchPlan q) { sbk::k8b_cuts_body(q); }
 __global__ void __launch_bounds__(128) k8b_blocks_kernel(sbk::RawBatchPlan q) { sbk::k8b_blocks_body(q); }
 __global__ void __launch_bounds__(128) k8b_finish_kernel(sbk::RawBatchPlan q) { sbk::k8b_finish_body(q); }
+__global__ void __launch_bounds__(128) k8b_validate_blocks_kernel(sbk::RawBatchPlan q) { sbk::k8b_blocks_body<false>(q); }
+__global__ void __launch_bounds__(128) k8b_validate_finish_kernel(sbk::RawBatchPlan q) { sbk::k8b_finish_body<false>(q); }
 __global__ void __launch_bounds__(256) k9_plan_kernel(sbk::RawCompressPlan q) { sbk::k9_plan_body(q); }
 __global__ void __launch_bounds__(1024) k9_scan_local_kernel(sbk::RawCompressPlan q) { sbk::k9_scan_local_body(q); }
 __global__ void __launch_bounds__(1024) k9_scan_tiles_kernel(sbk::RawCompressPlan q) { sbk::k9_scan_tiles_body(q); }
@@ -111,6 +114,8 @@ __global__ void __launch_bounds__(1024) k11_oscan_local_kernel(sbk::FrameDecodeB
 __global__ void __launch_bounds__(1024) k11_oscan_tiles_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_oscan_tiles_body(q); }
 __global__ void __launch_bounds__(128) k11_decode_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_decode_body(q); }
 __global__ void __launch_bounds__(256) k11_finish_kernel(sbk::FrameDecodeBatchPlan q) { sbk::k11_finish_body(q); }
+// with the occupancy hint ptxas keeps the chunk hand-out in registers across K2 and K3 (without it: 48 and a 16-byte spill)
+__global__ void __launch_bounds__(128, 4) k19_validate_kernel(sbk::FrameValidatePlan t) { sbk::k19_validate_body(t); }
 __global__ void __launch_bounds__(1024) k12_plan_kernel(sbk::RangePlan q) { sbk::k12_plan_body(q); }
 __global__ void __launch_bounds__(1024) k12_plan_tiles_kernel(sbk::RangePlan q) { sbk::k12_plan_tiles_body(q); }
 // with the occupancy hint ptxas keeps the pair lookup in registers across K5's decode (without it: 64 and a 4-byte spill)
@@ -651,6 +656,30 @@ int launch_raw_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_u
     CK(cudaGetLastError());
     return 0;
 }
+// The batch with its inputs and results only: no output pointers, and a cap no header exceeds (validation decides as a
+// decode into buffers of 2^32 - 1 bytes would).
+sb_batch validate_view(const sb_batch& b) {
+    sb_batch u;
+    memset(&u, 0, sizeof u);
+    u.in_ptrs = b.in_ptrs; u.in_base = b.in_base; u.in_stride = b.in_stride; u.in_lens = b.in_lens;
+    u.in_len_uniform = b.in_len_uniform; u.out_cap_uniform = 0xFFFFFFFFu;
+    u.out_lens = b.out_lens; u.statuses = b.statuses; u.count = b.count;
+    return u;
+}
+// K8b's sequence with the output-free block and one-warp passes
+int launch_raw_validate(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t* d_unit_blocks, void* scratch, cudaStream_t st,
+                        sb_error* err) {
+    if (b.count == 0) return 0;
+    const sbk::RawBatchPlan q = make_raw_batch_plan(validate_view(b), in_bytes, d_unit_blocks, scratch);
+    int rc = raw_batch_split(c, q, st, err);
+    if (rc) return rc;
+    k8b_validate_blocks_kernel<<<device_grid(c, q.in_bytes / 3072 + b.count, 4, 16), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    static const int per_sm = getenv("SNAPB200_K2_CTAS") ? atoi(getenv("SNAPB200_K2_CTAS")) : K8B_FINISH_CTAS_PER_SM;
+    k8b_validate_finish_kernel<<<device_grid(c, b.count, 4, per_sm), 128, 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
+    g_launches += 2;
+    CK(cudaGetLastError());
+    return 0;
+}
 
 
 // ---- raw batch compress (units of any length: every block of the batch in one K1 launch, assembled per unit)
@@ -828,6 +857,28 @@ int launch_frame_decode_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint
     // the payload part: decode + CRC, then the results
     k11_decode_kernel<<<device_grid(c, max_chunks, 4, 16), 128, sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP, st>>>(q);
     k11_finish_kernel<<<device_grid(c, b.count, 256, 16), 256, 0, st>>>(q);
+    g_launches += 2;
+    CK(cudaGetLastError());
+    return 0;
+}
+
+// ---- frame batch validation (K11's index part on the output-free view, K19's staged decode + CRC, K11's finish)
+uint64_t frame_validate_batch_ws_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks) {
+    return sbk::k19_carve(nullptr, count, in_bytes, max_chunks, nullptr);
+}
+int launch_frame_validate_batch(Ctx& c, const sb_batch& b, uint64_t in_bytes, uint32_t flags, const uint64_t* d_chunk_offs,
+                                const uint64_t* d_index_at, uint32_t max_chunks, uint32_t* d_unit_chunks, void* scratch,
+                                cudaStream_t st, sb_error* err) {
+    sbk::FrameValidatePlan t;
+    memset(&t, 0, sizeof t);
+    t.q = make_frame_decode_batch_plan(validate_view(b), in_bytes, flags, d_chunk_offs, d_index_at, max_chunks, d_unit_chunks,
+                                       scratch);
+    sbk::k19_carve(scratch, b.count, in_bytes, max_chunks, &t);
+    int rc = frame_decode_batch_index(c, t.q, st, err);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(t.next, 0, sizeof *t.next, st));
+    k19_validate_kernel<<<(t.nslots + 3) / 4, 128, sbk::K3_TABLE_BYTES + 4 * sbk::K2_SMEM_PER_WARP, st>>>(t);
+    k11_finish_kernel<<<device_grid(c, b.count, 256, 16), 256, 0, st>>>(t.q);
     g_launches += 2;
     CK(cudaGetLastError());
     return 0;
@@ -1175,6 +1226,22 @@ int sb_decompress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint
     return 0;
 }
 
+int sb_validate_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t* d_unit_blocks, void* scratch,
+                                uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if (!batch || !batch->out_lens || !batch->statuses || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K8B_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K8B_MAX_COUNT);
+    if (batch->count == 0) { ok(err); return 0; }
+    const uint64_t need = raw_batch_ws_bytes(batch->count, in_bytes);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_raw_validate(*c, *batch, in_bytes, d_unit_blocks, scratch, (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
 uint64_t sb_compress_batch_scratch_bytes(uint32_t count, uint64_t in_bytes) { return raw_compress_ws_bytes(count, in_bytes); }
 
 int sb_compress_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, void* scratch, uint64_t scratch_bytes, void* stream,
@@ -1269,6 +1336,30 @@ int sb_frame_decode_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, ui
     if (rc) return rc;
     rc = launch_frame_decode_batch(*c, *batch, in_bytes, flags, d_chunk_offs, d_index_at, max_chunks, d_unit_chunks, scratch,
                                    (cudaStream_t)stream, err);
+    if (rc) return rc;
+    ok(err);
+    return 0;
+}
+
+uint64_t sb_frame_validate_batch_scratch_bytes(uint32_t count, uint64_t in_bytes, uint32_t max_chunks) {
+    return frame_validate_batch_ws_bytes(count, in_bytes, max_chunks);
+}
+
+int sb_frame_validate_batch_device_ws(const sb_batch* batch, uint64_t in_bytes, uint32_t flags, const uint64_t* d_chunk_offs,
+                                      const uint64_t* d_index_at, uint32_t max_chunks, uint32_t* d_unit_chunks, void* scratch,
+                                      uint64_t scratch_bytes, void* stream, sb_error* err) {
+    if (!batch || !batch->out_lens || !batch->statuses || !scratch) return fail(err, SB_E_INVALID);
+    if (batch->count >= sbk::K11_MAX_COUNT) return fail(err, SB_E_INVALID, batch->count, sbk::K11_MAX_COUNT);
+    if (!d_chunk_offs != !d_index_at) return fail(err, SB_E_INVALID);
+    if (max_chunks == 0 || max_chunks > sbk::K11_MAX_CHUNKS) return fail(err, SB_E_INVALID, max_chunks, sbk::K11_MAX_CHUNKS);
+    if (batch->count == 0) { ok(err); return 0; }
+    const uint64_t need = frame_validate_batch_ws_bytes(batch->count, in_bytes, max_chunks);
+    if (scratch_bytes < need) return fail(err, SB_E_INVALID, scratch_bytes, need);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    rc = launch_frame_validate_batch(*c, *batch, in_bytes, flags, d_chunk_offs, d_index_at, max_chunks, d_unit_chunks, scratch,
+                                     (cudaStream_t)stream, err);
     if (rc) return rc;
     ok(err);
     return 0;
@@ -1580,6 +1671,40 @@ int sb_decompress(const uint8_t* in, size_t n, uint8_t* out, size_t cap, size_t*
     if (res->e.code) { if (err) *err = res->e; return (int)res->e.code; }
     if (res->len) CK(cudaMemcpy(out, l.compact[0].p, res->len, cudaMemcpyDeviceToHost));
     *out_n = res->len;
+    ok(err);
+    return 0;
+}
+
+int sb_validate(const uint8_t* in, size_t n, size_t* out_len, sb_error* err) {
+    if ((!in && n) || !out_len) return fail(err, SB_E_INVALID);
+    if (n == 0) return fail(err, SB_EMPTY);
+    if (n > SB_MAX_INPUT) return fail(err, SB_E_INVALID);
+    Ctx* c;
+    int rc = get_ctx(&c, err);
+    if (rc) return rc;
+    Lane& l = c->lane[LANE_DEC];
+    std::lock_guard<std::mutex> lk(l.mu);
+    const uint64_t ws = raw_batch_ws_bytes(1, n);
+    CK(l.in[0].need(n + 64));
+    CK(l.status[0].need(sizeof(sb_error) + 16));
+    CK(l.ws[0].need(ws));
+    rc = need_pinned(l, 4, 4096, err); if (rc) return rc;
+    CK(cudaMemcpyAsync(l.in[0].p, in, n, cudaMemcpyHostToDevice, l.s_compute));
+    // a batch of one on the validation path: K8 splits a stream of more than one block, or one warp checks it
+    sb_batch b;
+    memset(&b, 0, sizeof b);
+    b.in_base = l.in[0].as<uint8_t>(); b.in_len_uniform = (uint32_t)n;
+    b.statuses = l.status[0].as<sb_error>();
+    b.out_lens = (uint32_t*)((uint8_t*)l.status[0].p + sizeof(sb_error));
+    b.count = 1;
+    rc = launch_raw_validate(*c, b, n, nullptr, l.ws[0].p, l.s_compute, err);
+    if (rc) return rc;
+    struct Res { sb_error e; uint32_t len; uint32_t pad; };
+    Res* res = (Res*)l.pinned[4];
+    CK(cudaMemcpyAsync(res, l.status[0].p, sizeof(sb_error) + 8, cudaMemcpyDeviceToHost, l.s_compute));
+    CK(cudaStreamSynchronize(l.s_compute));
+    if (res->e.code) { if (err) *err = res->e; return (int)res->e.code; }
+    *out_len = res->len;
     ok(err);
     return 0;
 }
@@ -2180,6 +2305,11 @@ int snappy_uncompressed_length(const char* compressed, size_t compressed_length,
     sb_error e;
     if (!result || compressed_length == 0) return 1;
     return sb_decompress_len((const uint8_t*)compressed, compressed_length, result, &e) ? 1 : 0;
+}
+int snappy_validate_compressed_buffer(const char* compressed, size_t compressed_length) {
+    sb_error e;
+    size_t n = 0;
+    return sb_validate((const uint8_t*)compressed, compressed_length, &n, &e) ? 1 : 0;
 }
 
 #ifdef K1_PROFILE

@@ -4,7 +4,7 @@ import ctypes as C
 from . import _lib
 from .error import from_c
 from .raw import (HOST_BUILD_BYTES, _batch_encode, _check_ranges, _gather, _gathered, _host_streams, _ptr, _split,
-                  _stored_tables, _windows)
+                  _stored_tables, _validate_units, _windows)
 
 MAX_BLOCK_SIZE = 1 << 16                      # src/lib.rs:97
 MAX_COMPRESS_BLOCK_SIZE = 76490               # src/frame.rs:12
@@ -107,6 +107,36 @@ def decode_batch(streams) -> list:
             raise from_c(_lib.SbError(int(s[0] & 0xFFFFFFFF), 0, int(s[1]), int(s[2]), int(s[3])))
     back = t_out.cpu().numpy()
     return [back[o:o + k].tobytes() for o, k in zip(out_offs, caps)]
+
+
+def validate_batch(streams) -> list:
+    """Every stream checked as `FrameDecoder::new(stream).read_to_end()` would check it, CRCs included, without its
+    decoded bytes: one sb_frame_validate_batch_device_ws call on the current torch stream, with the chunk table sized
+    and retried as decode_batch does. Streams are bytes-like; they go to the device in one copy and only out_lens and the
+    statuses come back. Returns [(nbytes, error)]: the decoded length and None, or the bytes produced before the first
+    error and that error (returned, not raised)."""
+    import numpy as np
+    import torch
+    L = _lib.lib()
+    lens = [memoryview(s).nbytes for s in streams]
+
+    def run(b, in_bytes, t_res, stream):
+        def call(max_chunks):
+            need = L.sb_frame_validate_batch_scratch_bytes(b.count, in_bytes, max_chunks)
+            t_scr = torch.empty(need, dtype=torch.uint8, device=t_res.device)
+            e = _lib.SbError()
+            if L.sb_frame_validate_batch_device_ws(C.byref(b), in_bytes, 0, None, None, max_chunks, None, t_scr.data_ptr(),
+                                                   need, stream, C.byref(e)):
+                raise from_c(e)
+            return t_res.cpu().numpy()
+
+        at_st = (4 * b.count + 7) // 8 * 8
+        back = call(min(sum(n // 1024 + 2 for n in lens), MAX_BATCH_CHUNKS))
+        if any(int(s[0]) & 0xFFFFFFFF == 202 and int(s[2]) == 1 for s in back[at_st:].view(np.uint64).reshape(-1, 4)):
+            back = call(min(sum(n // 8 + 2 for n in lens), MAX_BATCH_CHUNKS))
+        return back
+
+    return _validate_units(streams, run)
 
 
 def decode_all(stream) -> bytes:

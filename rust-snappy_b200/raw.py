@@ -69,6 +69,16 @@ class Decoder:
         return bytes(buf[:n])
 
 
+def validate(data) -> int:
+    """The decoded length of a raw stream, found without decoding it into memory (sb_validate); raises exactly what
+    `Decoder().decompress_vec(data)` raises."""
+    p, keep = _ptr(data) if len(data) else (None, None)
+    n, e = C.c_size_t(0), _lib.SbError()
+    if _lib.lib().sb_validate(p, len(data), C.byref(n), C.byref(e)):
+        raise from_c(e)
+    return n.value
+
+
 def crc32c_masked(data) -> int:
     """crc32::CheckSummer::crc32c_masked (src/crc32.rs:35-38), computed on the GPU."""
     p, keep = _ptr(data) if len(data) else (None, None)
@@ -154,6 +164,62 @@ def compress_batch(units, tables=False):
     instead (sb_compress_batch_tabled_device_ws) and returns (streams, tables): every stream's raw seek table as
     bytes, what TableReader would build for it, ready to be stored beside it and given to TableReader(..., tables=)."""
     return _batch_encode(units, lambda n: max_compress_len(n) if n < 0xFFFFFFFF else 0, False, tables)
+
+
+def _validate_units(units, run):
+    """Uploads bytes-like units with their descriptors in one copy, makes the validation call run(batch, in_bytes,
+    results, stream) on the current torch stream (it returns the results' device tensor to read, or raises), and
+    returns [(nbytes, error or None)] from one download of out_lens and the statuses."""
+    import numpy as np
+    import torch
+    views = [np.frombuffer(u, dtype=np.uint8) for u in units]
+    count = len(views)
+    if count == 0:
+        return []
+    lens = [v.size for v in views]
+    in_offs = np.zeros(count, dtype=np.int64)
+    in_offs[1:] = np.cumsum(lens[:-1])
+    at_desc = (sum(lens) + 7) // 8 * 8                       # in_ptrs (u64), then in_lens (u32)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    t_in = torch.empty(at_desc + 12 * count, dtype=torch.uint8, device=dev)
+    host = np.zeros(at_desc + 12 * count, dtype=np.uint8)
+    for o, v in zip(in_offs, views):
+        host[o:o + v.size] = v
+    host[at_desc:at_desc + 8 * count] = (in_offs + t_in.data_ptr()).view(np.uint8)
+    host[at_desc + 8 * count:] = np.array(lens, dtype=np.uint32).view(np.uint8)
+    t_in.copy_(torch.from_numpy(host))
+    # out_lens (u32) and the statuses (sb_error, 32 bytes), 8-byte aligned
+    at_st = (4 * count + 7) // 8 * 8
+    t_res = torch.empty(at_st + 32 * count, dtype=torch.uint8, device=dev)
+    b = _lib.SbBatch()
+    b.in_ptrs, b.in_lens = t_in.data_ptr() + at_desc, t_in.data_ptr() + at_desc + 8 * count
+    b.out_lens, b.statuses, b.count = t_res.data_ptr(), t_res.data_ptr() + at_st, count
+    back = run(b, sum(lens), t_res, torch.cuda.current_stream(dev).cuda_stream)
+    out_lens = back[:4 * count].view(np.uint32)
+    res = []
+    for k, st in zip(out_lens, back[at_st:].view(np.uint64).reshape(count, 4)):
+        code = int(st[0] & 0xFFFFFFFF)
+        res.append((int(k), from_c(_lib.SbError(code, 0, int(st[1]), int(st[2]), int(st[3]))) if code else None))
+    return res
+
+
+def validate_batch(units) -> list:
+    """Every unit checked as `Decoder().decompress_vec(unit)` would check it, without its decoded bytes: one
+    sb_validate_batch_device_ws call on the current torch stream. Units are bytes-like; they go to the device in one
+    copy and only out_lens and the statuses come back. Returns [(nbytes, error)]: the decoded length and None, or 0 and
+    the error decompress_vec would raise (returned, not raised)."""
+    import torch
+    L = _lib.lib()
+
+    def run(b, in_bytes, t_res, stream):
+        need = L.sb_decompress_batch_scratch_bytes(b.count, in_bytes)
+        t_scr = torch.empty(need, dtype=torch.uint8, device=t_res.device)
+        e = _lib.SbError()
+        if L.sb_validate_batch_device_ws(C.byref(b), in_bytes, None, t_scr.data_ptr(), need, stream, C.byref(e)):
+            raise from_c(e)
+        return t_res.cpu().numpy()
+
+    return _validate_units(units, run)
 
 
 def _stored_tables(tables, lens, dev, magic, rec, records):
